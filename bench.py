@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Benchmark of the VTP hot path on B200 (contract: see the task brief / DESIGN.md §Measurement).
+"""Benchmark of the VTP hot path on H100 (see DESIGN.md §Measurement).
 
   python bench.py --gpus N --steps K --warmup W            our arm  (one rank per GPU under torchrun for N > 1)
   python bench.py --impl reference --gpus N --steps K ...  reference arm: the CPU restatement of the reference's step
@@ -36,18 +36,22 @@ def parse():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--model", default="small")
-    ap.add_argument("--batch", type=int, default=256, help="source images per GPU per step")
+    ap.add_argument("--batch", type=int, default=None,
+                    help="source images per GPU per step (default: 256, halved until the step fits 80 GB: VTP-Large 128)")
     ap.add_argument("--prototypes", type=int, default=65536)
     ap.add_argument("--cpu-batch", type=int, default=4, help="source images per step of the CPU baseline sample")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-lpips", action="store_true", help="reconstruction loss = L1 only")
     ap.add_argument("--graph", default="auto", choices=["auto", "on", "off"],
                     help="run the step as one captured CUDA graph (auto = on)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed step produced (loss vector, seeded sample of the updated fp32 parameters) "
+                         "as DIR/<name>.npy")
     return ap.parse_args()
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     def __init__(self, index: int):
         self.index, self.proc, self.lines = index, None, []
@@ -185,7 +189,7 @@ def workload_config(args, world: int, flops_per_image: float, image_groups=None)
            "losses": ["clip", "dino_local", "dino_global", "ibot", "rec_l1"] + ([] if args.no_lpips else ["rec_lpips"]),
            "lpips": (not args.no_lpips) and "VGG16 (frozen, seeded-random weights: pretrained ones need network), weight 1.0",
            "optimizer": "fused AdamW + EMA teacher, in the timed region",
-           "l2": "inputs (>1 GB/step) and activations far exceed the 126 MB L2; no reuse across steps",
+           "l2": "inputs (>1 GB/step) and activations far exceed the 50 MB L2; no reuse across steps",
            "parallelism": f"dp{world}", "flops_per_image": flops_per_image}
     if image_groups is not None:
         cfg["image_groups"] = image_groups
@@ -202,6 +206,10 @@ def main():
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
+    if args.batch is None:   # host arithmetic only (vtp_b200/memory.py): the largest of 256, 128, ... that fits 80 GB
+        from vtp_b200.config import preset
+        from vtp_b200.memory import fit_batch
+        args.batch = fit_batch(preset(args.model), 256, head_out_dim=args.prototypes, lpips=not args.no_lpips)
 
     if args.impl == "reference":
         if rank != 0:
@@ -240,8 +248,8 @@ def main():
     if world > 1:
         dist.init_process_group("nccl", device_id=dev)
     cfg = preset(args.model)
-    # VTP-Base/Large at 256 images per GPU: size the SSL / reconstruction image groups for the 180 GB of HBM
-    # (vtp_b200/memory.py; (0, 0) = whole batch in one pass, which is what VTP-Small uses)
+    # size the batch and the SSL / reconstruction image groups for the 80 GB of HBM (vtp_b200/memory.py; (0, 0) = whole
+    # batch in one pass, which is what VTP-Small uses)
     from vtp_b200.memory import suggest_chunks
     ssl_chunk, rec_chunk = suggest_chunks(cfg, args.batch, head_out_dim=args.prototypes, lpips=not args.no_lpips)
     tc = TrainConfig(head_out_dim=args.prototypes, ssl_chunk=ssl_chunk, rec_chunk=rec_chunk)
@@ -297,6 +305,15 @@ def main():
     ms = max_over_ranks(e0.elapsed_time(e1))
     launches = lib.LAUNCHES - l0
     log(f"device-resident: {ms / args.steps:.1f} ms/step")
+    if args.dump_outputs and rank == 0:
+        # what the last timed step produced: its loss vector and a fixed, seeded sample (2^20 entries, 4 MB) of the fp32
+        # master parameters it updated; inputs and weights are seeded, so two builds compare output for output
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "loss.npy"), loss.detach().float().cpu().numpy())
+        n = tr.store.n
+        idx = torch.randperm(n, generator=torch.Generator().manual_seed(0))[: min(n, 1 << 20)].sort().values
+        np.save(os.path.join(args.dump_outputs, "params_sample.npy"), tr.store.p[idx.to(dev)].float().cpu().numpy())
     # ---- end-to-end timing: pinned host inputs -> H2D -> step -> D2H of the loss vector, every step
     barrier()
     e2, e3 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -325,7 +342,7 @@ def main():
     ms_e2e = max_over_ranks(e2.elapsed_time(e3))
     log(f"end-to-end: {ms_e2e / args.steps:.1f} ms/step")
     clocks = sampler.stop() if rank == 0 else None
-    # ---- dominant kernel: the tcgen05 GEMM (gemm_kernel<256,4,NONE>), timed live on its largest recurring shape on the
+    # ---- dominant kernel: the wgmma GEMM (gemm_kernel<128,3,NONE>), timed live on its largest recurring shape on the
     #      hot path: the FFN fc1 projection of the SSL student pass (bias, bf16 out; the SwiGLU gate is a separate pass)
     Mg, Ng, Kg = 2 * B * 257, 2 * tr.hs, tr.D
     A = torch.randn(Mg, Kg, device=dev).to(torch.bfloat16)
@@ -345,14 +362,6 @@ def main():
     gemm_ms = g0.elapsed_time(g1) / reps
     gemm_tflops = 2.0 * Mg * Ng * Kg / (gemm_ms * 1e-3) / 1e12
     traffic, traffic_src = None, None
-    try:  # DRAM bytes of this very launch (same M, N, K) from the committed ncu --set full capture under profiles/ — ncu
-        # cannot run inside the timed bench, so the number is stamped with the capture it came from
-        with open(os.path.join(ROOT, "profiles", "gemm_fc1_traffic.json")) as f:
-            tj = json.load(f)
-        if tj.get("M") == Mg and tj.get("N") == Ng and tj.get("K") == Kg:
-            traffic, traffic_src = tj["dram_bytes"], tj.get("source", "profiles/gemm_fc1_traffic.json")
-    except Exception:
-        pass
 
     def shutdown():
         """Release the step graph BEFORE the NCCL communicator (NCCL cannot destroy a communicator whose collectives live in a
@@ -375,9 +384,10 @@ def main():
             peaks = json.load(f)
     except Exception:
         pass
-    peak_burst = peaks.get("bf16_tflops", 1590.0)
-    peak_sust = peaks.get("bf16_tflops_sustained", 1400.0)
-    src = "measured (MEASURED_PEAKS.json)" if peaks else "fallback (B200_PROFILING.md)"
+    # H100 SXM data sheet: 989 TFLOP/s dense BF16 at up to 700 W (a power-limited card reaches less)
+    peak_burst = peaks.get("bf16_tflops", 989.0)
+    peak_sust = peaks.get("bf16_tflops_sustained", 989.0)
+    src = "measured (MEASURED_PEAKS.json)" if peaks else "H100 SXM data sheet"
     fl = train_step_flops_per_image(cfg, K=args.prototypes, lpips=not args.no_lpips)
     imgs = B * world * args.steps
     value = imgs / (ms * 1e-3)
@@ -396,7 +406,7 @@ def main():
         "launch_mode": (f"one CUDA graph replay per step ({tr.graph_launches} kernels of libvtp_b200.so inside)" if use_graph
                         else "eager: one host launch per kernel"),
         "clocks": clocks,
-        "roofline": {"bound": "tensor", "kernel": f"vtp::gemm_kernel<256,4,NONE,cluster2,TMA-store epilogue> FFN fc1 GEMM M={Mg} N={Ng} K={Kg} (+bias, bf16 out), "
+        "roofline": {"bound": "tensor", "kernel": f"vtp::gemm_kernel<128,3,NONE,TMA-store epilogue> FFN fc1 GEMM M={Mg} N={Ng} K={Kg} (+bias, bf16 out), "
                                f"timed ISOLATED on synthetic operands after the step loop ({reps} launches, CUDA events)",
                      "achieved": gemm_tflops, "peak": peak_burst, "unit": "TFLOP/s", "frac": gemm_tflops / peak_burst,
                      "peak_source": src + " burst (kernel timed alone)", "traffic": traffic, "traffic_source": traffic_src,
@@ -411,13 +421,6 @@ def main():
         cb, _ = cpu_baseline(args, steps=2, warmup=1)   # ~20 s of CPU work on the box's 32 threads
         out["cpu_baseline"] = cb
         out["cpu_config1"] = cpu_config1()              # BASELINE configs[0]: the reference's own CPU-runnable case
-    extra = os.path.join(ROOT, "profiles", "extra_configs_r2.json")
-    if os.path.exists(extra):                           # BASELINE configs[2..4]: committed hardware runs of this round
-        try:
-            with open(extra) as f:
-                out["extra_configs"] = json.load(f)
-        except Exception:
-            pass
     print(json.dumps(out), flush=True)
     shutdown()
 

@@ -1,4 +1,4 @@
-"""`vtp.models.vtp_hf` (reference: vtp/models/vtp_hf/__init__.py:18-25) served by the sm_100a implementation."""
+"""`vtp.models.vtp_hf` (reference: vtp/models/vtp_hf/__init__.py:18-25) served by the sm_90a implementation."""
 import os
 import sys
 

@@ -1,5 +1,5 @@
 /*
- * vtp_b200.h — C ABI of the B200-native (sm_100a) VTP hot path.
+ * vtp_b200.h — C ABI of the H100-native (sm_90a) VTP hot path.
  *
  * This is the drop-in boundary (SURVEY.md §8b): the reference (MiniMax-AI/VTP) is pure Python/PyTorch and has no
  * FFI of its own, so the boundary is the set of fused stages that the reference's L1 layers dispatch to ATen for.
@@ -24,7 +24,7 @@ enum {
     VTP_OK = 0,
     VTP_ERR_ARG = -1,   /* bad argument / unsupported shape */
     VTP_ERR_CUDA = -2,  /* CUDA runtime / driver error */
-    VTP_ERR_ARCH = -3,  /* device is not sm_100 */
+    VTP_ERR_ARCH = -3,  /* device is not sm_90 */
 };
 enum { VTP_F32 = 0, VTP_BF16 = 1 };
 enum { VTP_ACT_NONE = 0, VTP_ACT_GELU = 1, VTP_ACT_SWIGLU8 = 2, VTP_ACT_ROPE = 3, VTP_ACT_RELU = 4 };
@@ -35,7 +35,7 @@ int vtp_version(void);
 int vtp_check_device(void);
 
 /* ------------------------------------------------------------------------------------------------------------
- * tcgen05 / TMA GEMM with fused epilogue:  out = epi( A · Bᵀ ),  bf16 operands, fp32 accumulation in TMEM.
+ * wgmma / TMA GEMM with fused epilogue:  out = epi( A · Bᵀ ),  bf16 operands, fp32 accumulation.
  * Replaces every nn.Linear / 1x1 nn.Conv2d / 16x16-stride-16 nn.Conv2d on the path:
  *   layers/attention.py:62,64,92,94 (qkv, proj)   layers/ffn.py:73-81 (w1,w2,w3)   layers/embeddings.py:58,64
  *   encoders/vision_transformer_bottleneck.py:30,66-79   decoders/pixel_decoder.py:108,138,157,160
@@ -126,7 +126,7 @@ int vtp_l2norm_fwd(const void* x, int x_dtype, void* y, int y_dtype, float* norm
 /* layers/attention.py:110-126 after RoPE (F.scaled_dot_product_attention, scale 1/8, head_dim 64) and the causal
  * nn.MultiheadAttention of layers/block.py:387-412.  qkv bf16 [B*T][3*H*64] packed [q|k|v] x [H][64]; out bf16
  * [B*T][H*64]; lse fp32 [B][H][T] optional (saved for backward).  `prefix` leading tokens (cls) are computed on CUDA
- * cores, the other T-prefix (<=256) tokens on tcgen05. */
+ * cores, the other T-prefix (<=256) tokens on wgmma. */
 int vtp_attention_fwd(const void* qkv, void* out, float* lse, int B, int T, int H, int prefix, int causal,
                       vtp_stream_t stream);
 /* same op on fp32 tensors (CUDA cores) for the fp32-accurate inference mode */

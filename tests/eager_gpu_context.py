@@ -1,6 +1,6 @@
-"""NOT a test (not collected): context number for DESIGN.md — the reference ALGORITHM as eager PyTorch on the same B200.
+"""NOT a test (not collected): context number for DESIGN.md — the reference ALGORITHM as eager PyTorch on the same H100.
 
-The reference is pure PyTorch (SURVEY.md §0: "the bar on the GPU is PyTorch eager on the same B200"): this script runs the
+The reference is pure PyTorch (SURVEY.md §0: "the bar on the GPU is PyTorch eager on the same H100"): this script runs the
 3-objective step of oracle/train_step.py — the reference's towers restated functionally + the restated losses + autograd +
 torch.optim.AdamW + EMA — on `cuda` under `torch.autocast(bfloat16)` with `F.scaled_dot_product_attention` (flash) for the
 attention, i.e. what a user gets from the reference's modules on this GPU: cuBLAS / cuDNN / SDPA kernels, one launch per

@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 GEMM (vtp_gemm_bf16) against a plain fp32 PyTorch reference of the same op."""
+"""GPU parity of the wgmma GEMM (vtp_gemm_bf16) against a plain fp32 PyTorch reference of the same op."""
 import math
 
 import pytest
@@ -153,17 +153,28 @@ def test_gemm_pixel_shuffle():
     assert _relerr(out, ref) < 2e-5
 
 
-@pytest.mark.parametrize("variant", ["default", "VTP_GEMM_G2", "VTP_GEMM_NO_FAST", "VTP_GEMM_NO_CLUSTER"])
+@pytest.mark.parametrize("variant", ["default", "VTP_GEMM_G2", "VTP_GEMM_NO_FAST", "VTP_GEMM_NO_CLUSTER", "a_mn", "b_mn"])
 @pytest.mark.parametrize("out_f32,resid,relu", [(False, False, False), (False, True, False), (True, False, False),
                                                 (True, True, False), (False, False, True)])
 @pytest.mark.parametrize("M,N,K", [(1000, 384, 384), (777, 1160, 200), (260, 2048, 1024), (129, 72, 64)])
 def test_gemm_fast_epilogue_modes(monkeypatch, variant, out_f32, resid, relu, M, N, K):
     """The lean TMA-store epilogue (bias, rounding point, optional same-dtype residual, ReLU) incl. M / N tails, in place
-    and out of place, on the multicast (default), cta_group::2, generic-epilogue and single-CTA kernel variants."""
-    if variant != "default":
+    and out of place, on the lean and the generic epilogue (VTP_GEMM_NO_FAST), and with an MN-major A or B operand
+    (64- and 128-wide tiles: N = 72 runs on 128, N <= 64 elsewhere).  VTP_GEMM_G2 / VTP_GEMM_NO_CLUSTER named the
+    pre-Hopper pair-tile and single-CTA forms; the library no longer reads them and those ids run the default kernel."""
+    if variant == "VTP_GEMM_NO_FAST":
         monkeypatch.setenv(variant, "1")
     r8 = lambda v: (v + 7) // 8 * 8
     A, W = _mk((M, r8(K)), 11)[:, :K], _mk((N, r8(K)), 12, 0.1)[:, :K]
+    opA, opW, kw = A, W, {}
+    if variant == "a_mn":   # A stored [K][M] (padded rows of 8)
+        opA = torch.zeros(K, r8(M), device="cuda", dtype=torch.bfloat16)
+        opA[:, :M] = A.t()
+        kw = dict(a_mn=True, lda=r8(M))
+    elif variant == "b_mn":
+        opW = torch.zeros(K, r8(N), device="cuda", dtype=torch.bfloat16)
+        opW[:, :N] = W.t()
+        kw = dict(b_mn=True, ldb=r8(N))
     bias = torch.randn(N, device="cuda")
     dt = torch.float32 if out_f32 else torch.bfloat16
     x = torch.randn(M, N, device="cuda").to(dt)
@@ -174,8 +185,8 @@ def test_gemm_fast_epilogue_modes(monkeypatch, variant, out_f32, resid, relu, M,
     for inplace in ([False, True] if resid else [False]):
         xin = x.clone()
         out = xin if inplace else torch.full((M, N), float("nan"), device="cuda", dtype=dt)
-        lib.gemm(A, W, out, M=M, N=N, K=K, bias=bias, resid=xin if resid else None,
-                 act=lib.ACT_RELU if relu else lib.ACT_NONE)
+        lib.gemm(opA, opW, out, M=M, N=N, K=K, bias=bias, resid=xin if resid else None,
+                 act=lib.ACT_RELU if relu else lib.ACT_NONE, **kw)
         torch.cuda.synchronize()
         assert torch.isfinite(out.float()).all()
         # one bf16 ulp of slack where the fp32 accumulation order flips the rounding point
@@ -183,13 +194,14 @@ def test_gemm_fast_epilogue_modes(monkeypatch, variant, out_f32, resid, relu, M,
         assert _relerr(out, ref) < 2e-3
 
 
-@pytest.mark.parametrize("variant", ["default", "VTP_GEMM_NO_N64_BRES"])
+@pytest.mark.parametrize("variant", ["default", "VTP_GEMM_NO_N64_BRES", "VTP_GEMM_NO_FAST"])
 @pytest.mark.parametrize("relu", [False, True])
 @pytest.mark.parametrize("M,K", [(40000, 32), (38000, 96), (50001, 576), (131072, 32)])
 def test_gemm_n64_resident_weights(monkeypatch, variant, relu, M, K):
-    """Tall 64-column GEMMs with K <= 576 (the VGG conv1_1 im2col form) take the resident-weight 64-wide kernel whose two
-    epilogue warp groups alternate tiles: K shorter than a k-block (zero fill), ragged last tile, many tiles per CTA."""
-    if variant != "default":
+    """Tall 64-column GEMMs with K <= 576 (the VGG conv1_1 im2col form) on 64-wide tiles, lean and generic epilogue: K shorter
+    than a k-block (zero fill), ragged last tile, many tiles per persistent CTA.  VTP_GEMM_NO_N64_BRES named the pre-Hopper
+    resident-weight form; the library no longer reads it and that id runs the default kernel."""
+    if variant == "VTP_GEMM_NO_FAST":
         monkeypatch.setenv(variant, "1")
     A, W = _mk((M, K), 21, 0.5), _mk((64, K), 22, 0.1)
     bias = torch.randn(64, device="cuda")

@@ -1,4 +1,4 @@
-"""GPU parity of the HBM-bound kernels and the tcgen05 attention against plain fp32 PyTorch references."""
+"""GPU parity of the HBM-bound kernels and the wgmma attention against plain fp32 PyTorch references."""
 import math
 import os
 
@@ -106,26 +106,25 @@ def _sdpa_ref(qkv, B, T, H, causal):
                                                   (4, 77, 6, 0, True), (2, 197, 12, 1, False), (2, 130, 2, 2, False),
                                                   (64, 257, 6, 1, False), (7, 50, 2, 0, False), (3, 64, 2, 1, False),
                                                   (100, 37, 6, 1, False), (300, 257, 6, 1, False)])
-@pytest.mark.parametrize("variant", ["rows4", "rows8", "pipe"])
+@pytest.mark.parametrize("variant", ["rows4", "rows8", "pipe", "no_lse", "VTP_ATTN_NO_PACK"])
 def test_attention_fwd(B, T, H, prefix, causal, variant, monkeypatch):
-    """rows4: one thread per query row; rows8: two threads per row, opt-in VTP_ATTN_FWD8=1 (attn_fwd8_kernel), measured
-    x0.94 of rows4 at B=512, T=257 (profiles/hbm_kernels_r1.md).  pipe: persistent ping-pong kernel (attention_pipe.cu) for
-    128 < HW <= 256 — first hardware run in round 2: bit-identical to rows4 and x1.11 faster (profiles/r2_first_hardware_pass.md),
-    the default for those shapes since (VTP_ATTN_FWD_PIPE=0 selects rows4)."""
-    if variant == "pipe":
-        if causal or not (128 < T - prefix <= 256) or (T - prefix) % 8:
-            pytest.skip("shape not handled by the persistent kernel (falls back to rows4)")
-    monkeypatch.setenv("VTP_ATTN_FWD_PIPE", "1" if variant == "pipe" else "0")
-    monkeypatch.setenv("VTP_ATTN_FWD8", "1" if variant == "rows8" else "0")
+    """attn_fwd_kernel<NKT>: one 128-key tile (HW <= 128) or two (128 < HW <= 256), cls / prefix rows on CUDA cores, causal
+    text shapes, packed multi-sequence tiles for T <= 64 (VTP_ATTN_NO_PACK=1: one sequence per tile), with and without the
+    saved log-sum-exp.  rows4 / rows8 / pipe are the ids of the three pre-Hopper forward kernels (one or two threads per
+    query row, persistent ping-pong); the Hopper build has the one kernel above, which all three ids run."""
+    if variant == "VTP_ATTN_NO_PACK":
+        monkeypatch.setenv(variant, "1")
     g = torch.Generator(device="cuda").manual_seed(B * 1000 + T)
     qkv = (torch.randn(B * T, 3 * H * 64, device="cuda", generator=g) * 1.5).to(BF)
     out = torch.full((B * T, H * 64), float("nan"), device="cuda", dtype=BF)
-    lse = torch.empty(B, H, T, device="cuda")
+    lse = None if variant == "no_lse" else torch.empty(B, H, T, device="cuda")
     lib.attention_fwd(qkv, out, B, T, H, prefix=prefix, causal=causal, lse=lse)
     torch.cuda.synchronize()
     ref = _sdpa_ref(qkv, B, T, H, causal)
     assert torch.isfinite(out.float()).all()
     assert _rel(out, ref) < 6e-3, _rel(out, ref)
+    if lse is None:
+        return
     q, k, _ = [t.transpose(1, 2).float() for t in qkv.view(B, T, 3, H, 64).unbind(2)]
     s = q @ k.transpose(-1, -2) * 0.125
     if causal:

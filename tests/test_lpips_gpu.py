@@ -1,4 +1,4 @@
-"""GPU parity of the LPIPS loss + image gradient (tcgen05 implicit-conv VGG16) against the CPU oracle restatement of
+"""GPU parity of the LPIPS loss + image gradient (wgmma implicit-conv VGG16) against the CPU oracle restatement of
 vtp/utils/lpips.py with identical (seeded random) VGG/lin weights."""
 import pytest
 import torch
@@ -53,7 +53,7 @@ def test_conv_mode_gemm_matches_conv2d():
 
 @pytest.mark.parametrize("variant", ["default", "VTP_GEMM_CONV_NO_FAST", "VTP_GEMM_CONV_NO_CLUSTER", "VTP_GEMM_CONV_BRES=0",
                                      "VTP_GEMM_CONV_BRES=1", "VTP_GEMM_CONV_BRES=2", "VTP_GEMM_CONV_HALO=0",
-                                     "VTP_GEMM_CONV_HALO=1"])
+                                     "VTP_GEMM_CONV_HALO=1", "ldo_pad", "ldo_pad_no_fast", "no_relu"])
 @pytest.mark.parametrize("B,H,W,Ci,Co,mask", [(1, 24, 16, 64, 64, False), (3, 8, 8, 128, 256, True), (2, 32, 32, 64, 64, True),
                                               (5, 16, 16, 256, 512, False), (1, 8, 8, 512, 512, True),
                                               (3, 40, 24, 64, 64, False), (2, 20, 12, 64, 64, True), (3, 256, 256, 64, 64, False),
@@ -61,37 +61,33 @@ def test_conv_mode_gemm_matches_conv2d():
                                               (3, 40, 24, 128, 128, True), (2, 128, 128, 128, 128, False), (1, 24, 16, 256, 128, True),
                                               (2, 128, 128, 128, 64, True), (1, 16, 16, 128, 64, False)])
 def test_conv_mode_variants(monkeypatch, variant, B, H, W, Ci, Co, mask):
-    """Implicit 3x3 conv GEMM through the TMA-store epilogue (4-D NHWC tensor map) on clustered / single-CTA kernels:
-    odd tile counts (padded pair tile), Cout < tile width, bias+ReLU forward form and masked dgrad form; the 64 -> 64
-    channel shapes also through the resident-weight (BRES=1) and halo-block (BRES=2) forms (many tiles per CTA at 256 x 256,
-    ragged heights, W = 12 falls back from the halo form); the other shapes with tiles <= 128 wide through the two-ring halo
-    form (HALO=1: one to four 64-channel blocks, 64- and 128-wide tiles, odd pair counts)."""
-    if "BRES=" in variant:
-        if (Ci, Co) != (64, 64):
-            pytest.skip("resident-weight forms only exist for 64 -> 64 channels")
-        monkeypatch.setenv(*variant.split("="))
-    elif "HALO=" in variant:
-        if (Ci, Co) == (64, 64) or Co > 128:
-            pytest.skip("two-ring halo form: tiles <= 128 wide, not the 64 -> 64 shapes")
-        monkeypatch.setenv(*variant.split("="))
-    elif variant != "default":
-        monkeypatch.setenv(variant, "1")
+    """Implicit 3x3 conv GEMM (4-D TMA over NHWC, zero fill = padding) through the TMA-store epilogue (4-D NHWC tensor map)
+    and the generic one (VTP_GEMM_CONV_NO_FAST): 64- and 128-wide tiles, 16 / 8 / 4-pixel tile rows, ragged heights, Cout <
+    tile width, many tiles per persistent CTA, bias+ReLU forward form, bias-only form and masked dgrad form, and an output
+    whose pixel stride is wider than Cout (ldo_pad: the result lands in a channel slice of a wider NHWC buffer).  The
+    CONV_NO_CLUSTER / CONV_BRES / CONV_HALO ids named pre-Hopper conv forms; the library no longer reads them and those ids
+    run the default kernel."""
+    if variant in ("VTP_GEMM_CONV_NO_FAST", "ldo_pad_no_fast"):
+        monkeypatch.setenv("VTP_GEMM_CONV_NO_FAST", "1")
+    ldo = Co + 64 if variant.startswith("ldo_pad") else Co
     g = torch.Generator(device="cuda").manual_seed(B * 100 + Ci)
     x = (torch.randn(B, H, W, Ci, device="cuda", generator=g) * 0.5).to(torch.bfloat16)
     w = (torch.randn(Co, Ci, 3, 3, device="cuda", generator=g) * (2.0 / (9 * Ci)) ** 0.5).to(torch.bfloat16)
     wk = w.permute(0, 2, 3, 1).reshape(Co, 9 * Ci).contiguous()
-    y = torch.full((B, H, W, Co), float("nan"), device="cuda", dtype=torch.bfloat16)
+    ybuf = torch.full((B, H, W, ldo), float("nan"), device="cuda", dtype=torch.bfloat16)
+    y = ybuf[..., :Co]
     conv = torch.nn.functional.conv2d(x.float().permute(0, 3, 1, 2), w.float(), None, padding=1).permute(0, 2, 3, 1)
     if mask:
         m = torch.randn(B, H, W, Co, device="cuda", generator=g).to(torch.bfloat16)
-        lib.gemm(x, wk, y, M=B * H * W, N=Co, K=9 * Ci, lda=Ci, ldb=9 * Ci, ldo=Co, conv=(Ci, H, W), round_bf16=False,
+        lib.gemm(x, wk, ybuf, M=B * H * W, N=Co, K=9 * Ci, lda=Ci, ldb=9 * Ci, ldo=ldo, conv=(Ci, H, W), round_bf16=False,
                  mask_pos=m)
         ref = conv * (m.float() > 0)
     else:
         b = torch.randn(Co, device="cuda", generator=g) * 0.1
-        lib.gemm(x, wk, y, M=B * H * W, N=Co, K=9 * Ci, lda=Ci, ldb=9 * Ci, bias=b, act=lib.ACT_RELU, ldo=Co,
-                 conv=(Ci, H, W))
-        ref = torch.relu(conv + b)
+        relu = variant != "no_relu"
+        lib.gemm(x, wk, ybuf, M=B * H * W, N=Co, K=9 * Ci, lda=Ci, ldb=9 * Ci, bias=b, act=lib.ACT_RELU if relu else lib.ACT_NONE,
+                 ldo=ldo, conv=(Ci, H, W))
+        ref = torch.relu(conv + b) if relu else conv + b
     torch.cuda.synchronize()
     assert torch.isfinite(y.float()).all()
     assert rel(y, ref) < 5e-3, rel(y, ref)

@@ -1,12 +1,14 @@
 """HBM budget model of the training step (vtp_b200/memory.py) — host logic, no GPU."""
+import pytest
+
 from vtp_b200 import memory as m
 from vtp_b200.config import preset
 
 
 def test_small_matches_the_measured_peak():
-    """profiles/bench_n2_r1.log: VTP-Small, 256 images/GPU, K = 65536 -> 41.7 GiB peak (torch.cuda.max_memory_allocated)."""
+    """Measured on an H100: VTP-Small, 256 images/GPU, K = 65536 -> 42.7 GiB peak (torch.cuda.max_memory_allocated)."""
     est = m.train_step_bytes(preset("small"), 256)
-    assert abs(est["peak"] / m.GIB - 41.7) < 0.15 * 41.7
+    assert abs(est["peak"] / m.GIB - 42.7) < 0.15 * 42.7
     assert est["ssl"] > est["rec"] > est["clip"]
     assert abs(est["params"] / 1e6 - 106.2) < 1.0          # SURVEY §8d: 83.8 M model + ~22.3 M DINO head
 
@@ -14,12 +16,19 @@ def test_small_matches_the_measured_peak():
 def test_large_needs_chunks_and_chunks_fit():
     cfg = preset("large")
     est = m.train_step_bytes(cfg, 256)
-    assert est["peak"] > 180e9                               # config 4 does not fit a B200 in one piece
-    ssl_chunk, rec_chunk = m.suggest_chunks(cfg, 256, budget_bytes=150 * m.GIB)
-    assert 0 < ssl_chunk < 256
-    fit = m.train_step_bytes(cfg, 256, ssl_chunk=ssl_chunk, rec_chunk=rec_chunk)
-    assert fit["peak"] <= 150 * m.GIB
-    assert m.suggest_chunks(preset("small"), 256) == (0, 0) and m.suggest_chunks(preset("base"), 256) == (0, 0)
+    assert est["peak"] > 80e9                                # config 4 does not fit an H100 in one piece
+    with pytest.raises(ValueError):                           # 256 per GPU: the contrastive pass alone exceeds 64 GiB
+        m.suggest_chunks(cfg, 256)
+    B = m.fit_batch(cfg, 256)                                 # what bench.py runs for VTP-Large on an 80 GB H100
+    assert B == 128
+    ssl_chunk, rec_chunk = m.suggest_chunks(cfg, B)
+    assert 0 < ssl_chunk < B
+    fit = m.train_step_bytes(cfg, B, ssl_chunk=ssl_chunk, rec_chunk=rec_chunk)
+    assert fit["peak"] <= 64 * m.GIB
+    assert m.fit_batch(preset("small"), 256) == 256 and m.fit_batch(preset("base"), 256) == 256
+    assert m.suggest_chunks(preset("small"), 256) == (0, 0)               # VTP-Small runs in one piece on 80 GB
+    bs, br = m.suggest_chunks(preset("base"), 256)
+    assert m.train_step_bytes(preset("base"), 256, ssl_chunk=bs, rec_chunk=br)["peak"] <= 64 * m.GIB
 
 
 def test_tape_bytes_formula():

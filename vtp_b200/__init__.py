@@ -1,4 +1,4 @@
-"""vtp_b200 — B200-native (sm_100a) implementation of the MiniMax-AI/VTP hot path behind the reference's own API."""
+"""vtp_b200 — H100-native (sm_90a) implementation of the MiniMax-AI/VTP hot path behind the reference's own API."""
 from .config import VTPConfig, preset  # noqa: F401
 
 

@@ -1,4 +1,4 @@
-"""Build the in-tree C-ABI shared library `vtp_b200/libvtp_b200.so` with nvcc for sm_100a.
+"""Build the in-tree C-ABI shared library `vtp_b200/libvtp_b200.so` with nvcc for sm_90a.
 
 No torch involvement: plain `nvcc -shared`, objects cached per source by mtime. Also builds oracle/ C checkers if
 present.  Usage:  python -m vtp_b200.build [--force] [--verbose]
@@ -17,7 +17,7 @@ LIB_PATH = os.path.join(HERE, "libvtp_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",

@@ -1,16 +1,16 @@
-// vtp_b200 — fused self-attention forward for short sequences (T = prefix + HW, HW <= 256) on tcgen05.
+// vtp_b200 — fused self-attention forward for short sequences (T = prefix + HW, HW <= 256) on wgmma.
 //
 // Replaces layers/attention.py:110-126 (SelfAttention.compute_attention after RoPE: SDPA with scale 1/sqrt(64), no
 // mask, no dropout) and nn.MultiheadAttention's causal SDPA in the text tower (layers/block.py:387-412).
 //
-// One CTA per (query tile of 128 patch rows, head, image); 2 CTAs/SM (112 KB smem, 256 TMEM columns each).
-//   S = Q·Kᵀ     one UMMA chain  M=128, N=128|256, K=64      (Q,K tiles by TMA straight out of the packed qkv buffer)
-//   softmax      one thread per query row, the whole row lives in TMEM -> exact single-pass softmax (no online rescale)
-//   O = P·V      P written as bf16 into a swizzled K-major smem tile in two 128-key halves, V consumed as an MN-major
-//                B operand (no transpose); O accumulates in TMEM columns [0,64) that S no longer needs.
+// One CTA per (query tile of 128 patch rows, head, image): two consumer warpgroups of 64 query rows each and one extra warp.
+//   S = Q·Kᵀ     one wgmma chain per warpgroup  m64 x N=128|256 x K=64  (Q,K tiles by TMA straight out of the packed qkv
+//                buffer); the whole score row lives in the registers of one thread quad -> exact single-pass softmax
+//   O = P·V      P is re-packed in registers as the bf16 A operand (no shared-memory round trip), V is consumed as an
+//                MN-major B operand (no transpose)
 // The `prefix` (cls / storage) tokens — 1 in the encoder, 0 in the decoder/text — would cost a third 128-row tile for
 // one row, so they are handled on CUDA cores: their key columns are folded into every row's softmax by the row
-// threads, and their query rows are computed by a spare warp from the K/V tiles already in smem.
+// threads, and their query rows are computed by the extra warp from the K/V tiles already in smem.
 #include <stdlib.h>
 
 #include "attention.h"
@@ -19,12 +19,12 @@
 
 namespace vtp {
 
-static constexpr int ATT_THREADS = 192;
+static constexpr int ATT_THREADS = 384;  // 2 consumer warpgroups + warpgroup 2 (warp 8: TMA, prefix query rows)
 static constexpr int MAX_PREFIX = ATT_MAX_PREFIX;
-// smem: Q 16K | K 32K | V 32K | P 32K | barriers
-static constexpr int SQ = 0, SK = 16384, SV = SK + 32768, SP = SV + 32768, SBAR = SP + 32768;
-static constexpr int SPCLS = SBAR + 128;      // bf16 [256]: softmax numerators of the cls query row (warp 5)
-static constexpr int ATT_SMEM = SPCLS + 512;  // 115328 B -> 2 CTAs/SM
+// smem: Q 16K | K 32K | V 32K | barriers
+static constexpr int SQ = 0, SK = 16384, SV = SK + 32768, SBAR = SV + 32768;
+static constexpr int SPCLS = SBAR + 128;      // bf16 [256]: softmax numerators of the cls query row (warp 8)
+static constexpr int ATT_SMEM = SPCLS + 512 + 1024;  // + alignment slack
 
 __device__ __forceinline__ float ex2f(float x) {  // ex2.approx.ftz (ex2f() carries a 4-instruction denormal slow path)
     float y;
@@ -35,18 +35,14 @@ __device__ __forceinline__ uint32_t sw128_off(int row, int col /*bf16 element 0.
     return row * 128 + ((((col >> 3) ^ (row & 7)) << 4) | ((col & 7) << 1));
 }
 
-__global__ void __launch_bounds__(ATT_THREADS, 2) attn_fwd_kernel(const __grid_constant__ CUtensorMap tm, const AttnDev p) {
-    extern __shared__ __align__(1024) uint8_t smem[];
-    if (smem_u32(smem) & 1023) __trap();  // SWIZZLE_128B tiles need a 1024B-aligned base
+template <int NKT>
+__global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_kernel(const __grid_constant__ CUtensorMap tm, const AttnDev p) {
+    constexpr int NK = 128 * NKT;  // key columns of S
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SBAR);
-    uint64_t* bar_qk = bars + 0;   // Q,K landed
-    uint64_t* bar_v = bars + 1;    // V landed
-    uint64_t* bar_s = bars + 2;    // S complete in TMEM
-    uint64_t* bar_p0 = bars + 3;   // P half 0 written (128 arrivals)
-    uint64_t* bar_pv0 = bars + 4;  // PV half 0 done (P buffer reusable)
-    uint64_t* bar_p1 = bars + 5;   // P half 1 written
-    uint64_t* bar_o = bars + 6;    // O complete
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
+    uint64_t* bar_qk = bars + 0;  // Q,K landed
+    uint64_t* bar_v = bars + 1;   // V landed
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     // packed mode (short sequences, e.g. the 37-token local crops): the tile holds `pack` consecutive sequences, every
@@ -54,209 +50,177 @@ __global__ void __launch_bounds__(ATT_THREADS, 2) attn_fwd_kernel(const __grid_c
     const int qt = blockIdx.x, h = blockIdx.y, b = p.pack ? blockIdx.z * p.pack : blockIdx.z;
     const int D = p.D, T = p.T, prefix = p.prefix, HW = p.HW;
     const long seq_row0 = (long)b * T;
-    const int kvrows = 128 * p.nkt;
+    const int kvrows = NK;
 
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&tm);
-        mbar_init(bar_qk, 1), mbar_init(bar_v, 1), mbar_init(bar_s, 1), mbar_init(bar_p0, 128);
-        mbar_init(bar_pv0, 1), mbar_init(bar_p1, 128), mbar_init(bar_o, 1);
+        mbar_init(bar_qk, 1), mbar_init(bar_v, 1);
         fence_barrier_init();
     }
-    if (warp == 0) {
-        tmem_alloc(tmem_slot, 256);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp < 8) {
+        // ---------------- consumers: thread quad (lane / 4) of warp w owns query rows 16 w + lane / 4 (+ 8)
+        setmaxnreg_inc<200>();  // 384 x 168 registers: + 256 x 32 here = - 128 x 64 in warpgroup 2
+        const int wg = warp >> 2, tw = threadIdx.x & 127, c4 = lane & 3;
+        int rr[2], qpos[2], qtok[2], pseq[2], kmin[2], kmax[2];
+        bool row_valid[2];
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            rr[i] = 64 * wg + 16 * (tw >> 5) + (lane >> 2) + 8 * i;  // row within the tile
+            qpos[i] = 128 * qt + rr[i];                              // patch index of this query
+            qtok[i] = prefix + qpos[i];                              // token index within the sequence
+            pseq[i] = p.pack ? rr[i] / T : 0;                        // packed mode: my sequence within the tile
+            row_valid[i] = p.pack ? (pseq[i] < p.pack && b + pseq[i] < p.B) : (qpos[i] < HW);
+            // keys [kmin,kmax) are visible
+            kmin[i] = p.pack ? (row_valid[i] ? pseq[i] * T : 0) : 0;
+            kmax[i] = p.pack ? (row_valid[i] ? kmin[i] + T : 0) : (p.causal ? min(HW, qpos[i] + 1) : HW);
+        }
+        mbar_wait(bar_qk, 0);
+        float s[NK / 2];
+        {
+            const uint32_t qa = smem_u32(smem + SQ) + wg * 8192, ka = smem_u32(smem + SK);
+            wgmma_fence();
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const uint64_t ad = wgmma_desc_sw128(qa + j * 32, 0, 1024), bd = wgmma_desc_sw128(ka + j * 32, 0, 1024);
+                if constexpr (NKT == 2) wgmma_m64n256_ss<0, 0>(s, ad, bd, j > 0);
+                else wgmma_m64n128_ss<0, 0>(s, ad, bd, j > 0);
+            }
+            wgmma_commit();
+        }
+        // scores against the prefix keys (CUDA cores, while the MMAs run): q rows from smem (swizzled), k rows from
+        // global; the four threads of the quad take 16 dims each
+        float s_pre[2][MAX_PREFIX];
+#pragma unroll
+        for (int j = 0; j < MAX_PREFIX; ++j) {
+            float acc0 = 0.f, acc1 = 0.f;
+            if (j < prefix) {
+                const uint4* kp = reinterpret_cast<const uint4*>(p.qkv + (seq_row0 + j) * 3 * D + D + h * 64 + 16 * c4);
+#pragma unroll
+                for (int c = 0; c < 2; ++c) {
+                    const uint4 w = __ldg(kp + c);
+                    const uint4 q0 = *reinterpret_cast<const uint4*>(smem + SQ + sw128_off(rr[0], 16 * c4 + 8 * c));
+                    const uint4 q1 = *reinterpret_cast<const uint4*>(smem + SQ + sw128_off(rr[1], 16 * c4 + 8 * c));
+                    const uint32_t kw[4] = {w.x, w.y, w.z, w.w}, qw0[4] = {q0.x, q0.y, q0.z, q0.w}, qw1[4] = {q1.x, q1.y, q1.z, q1.w};
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) {
+                        acc0 += bf16_lo(qw0[e]) * bf16_lo(kw[e]) + bf16_hi(qw0[e]) * bf16_hi(kw[e]);
+                        acc1 += bf16_lo(qw1[e]) * bf16_lo(kw[e]) + bf16_hi(qw1[e]) * bf16_hi(kw[e]);
+                    }
+                }
+            }
+            acc0 += __shfl_xor_sync(0xffffffffu, acc0, 1), acc1 += __shfl_xor_sync(0xffffffffu, acc1, 1);
+            acc0 += __shfl_xor_sync(0xffffffffu, acc0, 2), acc1 += __shfl_xor_sync(0xffffffffu, acc1, 2);
+            s_pre[0][j] = (j < prefix && (!p.causal || j <= qtok[0])) ? acc0 : -INFINITY;
+            s_pre[1][j] = (j < prefix && (!p.causal || j <= qtok[1])) ? acc1 : -INFINITY;
+        }
+        wgmma_wait<0>();
+        fence_regs(s);
+        // pass 1: row max (score s[4 jn + 2 i + c] is key 8 jn + 2 c4 + c of row i)
+        float m[2], msc[2], l[2];
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            m[i] = -INFINITY;
+#pragma unroll
+            for (int j = 0; j < MAX_PREFIX; ++j) m[i] = fmaxf(m[i], s_pre[i][j]);
+        }
+#pragma unroll
+        for (int jn = 0; jn < NK / 8; ++jn)
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+#pragma unroll
+                for (int c = 0; c < 2; ++c) {
+                    const int key = 8 * jn + 2 * c4 + c;
+                    if (key >= kmin[i] && key < kmax[i]) m[i] = fmaxf(m[i], s[4 * jn + 2 * i + c]);
+                }
+        float p_pre[2][MAX_PREFIX];
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            m[i] = fmaxf(m[i], __shfl_xor_sync(0xffffffffu, m[i], 1));
+            m[i] = fmaxf(m[i], __shfl_xor_sync(0xffffffffu, m[i], 2));
+            msc[i] = (m[i] == -INFINITY) ? 0.f : m[i] * p.scale_log2;
+            l[i] = 0.f;
+#pragma unroll
+            for (int j = 0; j < MAX_PREFIX; ++j) {
+                p_pre[i][j] = (s_pre[i][j] == -INFINITY) ? 0.f : ex2f(s_pre[i][j] * p.scale_log2 - msc[i]);
+                if (c4 == 0) l[i] += p_pre[i][j];  // the prefix columns are counted once per row (quad sum below)
+                p_pre[i][j] = bf16_round(p_pre[i][j]);
+            }
+        }
+        // pass 2: p = exp2(s*scale*log2e - m*scale*log2e) in place, the bf16 numerators feed P·V from registers
+#pragma unroll
+        for (int jn = 0; jn < NK / 8; ++jn)
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+#pragma unroll
+                for (int c = 0; c < 2; ++c) {
+                    const int key = 8 * jn + 2 * c4 + c;
+                    float& v = s[4 * jn + 2 * i + c];
+                    v = (key >= kmin[i] && key < kmax[i]) ? ex2f(v * p.scale_log2 - msc[i]) : 0.f;
+                    l[i] += v;
+                }
+        mbar_wait(bar_v, 0);
+        float o[32];
+        {
+            const uint32_t va = smem_u32(smem + SV);
+            wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < NK / 16; ++kk) {  // 16 keys per k-step
+                const uint32_t a[4] = {pack_bf16x2(s[8 * kk], s[8 * kk + 1]), pack_bf16x2(s[8 * kk + 2], s[8 * kk + 3]),
+                                       pack_bf16x2(s[8 * kk + 4], s[8 * kk + 5]), pack_bf16x2(s[8 * kk + 6], s[8 * kk + 7])};
+                wgmma_m64n64_rs<1>(o, a, wgmma_desc_sw128(va + kk * 2048, 8192, 1024), kk > 0);
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs(o);
+        }
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            l[i] += __shfl_xor_sync(0xffffffffu, l[i], 1);
+            l[i] += __shfl_xor_sync(0xffffffffu, l[i], 2);
+        }
+        // epilogue: o[4 jn + 2 i + c] is dim 8 jn + 2 c4 + c of row i
+#pragma unroll
+        for (int j = 0; j < MAX_PREFIX; ++j) {
+            if (j < prefix) {
+                const __nv_bfloat16* vp = p.qkv + (seq_row0 + j) * 3 * D + 2 * D + h * 64 + 2 * c4;
+#pragma unroll
+                for (int jn = 0; jn < 8; ++jn) {
+                    const uint32_t w = __ldg(reinterpret_cast<const uint32_t*>(vp + 8 * jn));
+#pragma unroll
+                    for (int i = 0; i < 2; ++i)
+                        o[4 * jn + 2 * i] += p_pre[i][j] * bf16_lo(w), o[4 * jn + 2 * i + 1] += p_pre[i][j] * bf16_hi(w);
+                }
+            }
+        }
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            if (!row_valid[i]) continue;
+            const float inv = 1.f / l[i];
+            __nv_bfloat16* op = p.out + (seq_row0 + qtok[i]) * D + h * 64 + 2 * c4;
+#pragma unroll
+            for (int jn = 0; jn < 8; ++jn)
+                *reinterpret_cast<uint32_t*>(op + 8 * jn) = pack_bf16x2(o[4 * jn + 2 * i] * inv, o[4 * jn + 2 * i + 1] * inv);
+            if (p.lse && c4 == 0) {
+                if (p.pack) p.lse[((long)(b + pseq[i]) * p.H + h) * T + (rr[i] - pseq[i] * T)] = m[i] * p.scale + logf(l[i]);
+                else p.lse[((long)b * p.H + h) * T + qtok[i]] = m[i] * p.scale + logf(l[i]);
+            }
+        }
+    } else {
+        setmaxnreg_dec<104>();
+        if (warp != 8) return;
         if (lane == 0) {
             // ---------------- TMA
             const int row_q = (int)seq_row0 + prefix + 128 * qt;
             const int row_k = (int)seq_row0 + prefix;
-            mbar_expect_tx(bar_qk, 16384 + 16384 * p.nkt);
+            mbar_expect_tx(bar_qk, 16384 + 16384 * NKT);
             tma_load_2d(smem + SQ, &tm, bar_qk, h * 64, row_q);
-            for (int i = 0; i < p.nkt; ++i) tma_load_2d(smem + SK + i * 16384, &tm, bar_qk, D + h * 64, row_k + 128 * i);
-            mbar_expect_tx(bar_v, 16384 * p.nkt);
-            for (int i = 0; i < p.nkt; ++i)
-                tma_load_2d(smem + SV + i * 16384, &tm, bar_v, 2 * D + h * 64, row_k + 128 * i);
-            // ---------------- S = Q Kᵀ
-            mbar_wait(bar_qk, 0);
-            tc_fence_after();
-            const uint32_t idesc_s = umma_idesc_bf16(128, kvrows, 0, 0);
-            const uint32_t qa = smem_u32(smem + SQ), ka = smem_u32(smem + SK);
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-                umma_bf16_ss(tmem, umma_desc_sw128(qa + j * 32, 0, 1024), umma_desc_sw128(ka + j * 32, 0, 1024), idesc_s,
-                             j > 0);
-            umma_commit(bar_s);
-            // ---------------- O = P V  (two 128-key halves through one P buffer)
-            const uint32_t idesc_o = umma_idesc_bf16(128, 64, 0, 1);  // B (=V) is MN-major
-            const uint32_t pa = smem_u32(smem + SP), va = smem_u32(smem + SV);
-            mbar_wait(bar_v, 0);
-            for (int half = 0; half < p.nkt; ++half) {
-                mbar_wait(half == 0 ? bar_p0 : bar_p1, 0);
-                tc_fence_after();
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {  // 8 k-steps of 16 keys
-                    const uint64_t ad = umma_desc_sw128(pa + (j >> 2) * 16384 + (j & 3) * 32, 0, 1024);
-                    const uint64_t bd = umma_desc_sw128(va + half * 16384 + j * 2048, 8192, 1024);
-                    umma_bf16_ss(tmem, ad, bd, idesc_o, (half > 0 || j > 0) ? 1u : 0u);
-                }
-                umma_commit(half == 0 && p.nkt == 2 ? bar_pv0 : bar_o);
-            }
+            for (int i = 0; i < NKT; ++i) tma_load_2d(smem + SK + i * 16384, &tm, bar_qk, D + h * 64, row_k + 128 * i);
+            mbar_expect_tx(bar_v, 16384 * NKT);
+            for (int i = 0; i < NKT; ++i) tma_load_2d(smem + SV + i * 16384, &tm, bar_v, 2 * D + h * 64, row_k + 128 * i);
         }
-    } else if (warp <= 4) {
-        // ---------------- softmax + epilogue: one thread per query row
-        const int q4 = warp & 3;
-        const int r = q4 * 32 + lane;             // row within the tile == TMEM lane
-        const int qpos = 128 * qt + r;            // patch index of this query
-        const int qtok = prefix + qpos;           // token index within the sequence
-        const int pseq = p.pack ? r / T : 0;  // packed mode: my sequence within the tile
-        const bool row_valid = p.pack ? (pseq < p.pack && b + pseq < p.B) : (qpos < HW);
-        const uint32_t trow = tmem + (uint32_t(q4 * 32) << 16);
-
-        // scores against the prefix keys (CUDA cores): q row from smem (swizzled), k rows from global
-        float s_pre[MAX_PREFIX];
-        mbar_wait(bar_qk, 0);
-        if (prefix > 0) {
-            float qf[64];
-#pragma unroll
-            for (int c = 0; c < 8; ++c) {
-                const uint4 w = *reinterpret_cast<const uint4*>(smem + SQ + sw128_off(r, c * 8));
-                qf[c * 8 + 0] = bf16_lo(w.x), qf[c * 8 + 1] = bf16_hi(w.x), qf[c * 8 + 2] = bf16_lo(w.y);
-                qf[c * 8 + 3] = bf16_hi(w.y), qf[c * 8 + 4] = bf16_lo(w.z), qf[c * 8 + 5] = bf16_hi(w.z);
-                qf[c * 8 + 6] = bf16_lo(w.w), qf[c * 8 + 7] = bf16_hi(w.w);
-            }
-#pragma unroll
-            for (int j = 0; j < MAX_PREFIX; ++j) {
-                s_pre[j] = -INFINITY;
-                if (j < prefix) {
-                    const uint4* kp = reinterpret_cast<const uint4*>(p.qkv + (seq_row0 + j) * 3 * D + D + h * 64);
-                    float acc = 0.f;
-#pragma unroll
-                    for (int c = 0; c < 8; ++c) {
-                        const uint4 w = __ldg(kp + c);
-                        acc += qf[c * 8 + 0] * bf16_lo(w.x) + qf[c * 8 + 1] * bf16_hi(w.x) + qf[c * 8 + 2] * bf16_lo(w.y) +
-                               qf[c * 8 + 3] * bf16_hi(w.y) + qf[c * 8 + 4] * bf16_lo(w.z) + qf[c * 8 + 5] * bf16_hi(w.z) +
-                               qf[c * 8 + 6] * bf16_lo(w.w) + qf[c * 8 + 7] * bf16_hi(w.w);
-                    }
-                    if (!p.causal || j <= qtok) s_pre[j] = acc;
-                }
-            }
-        } else {
-#pragma unroll
-            for (int j = 0; j < MAX_PREFIX; ++j) s_pre[j] = -INFINITY;
-        }
-
-        mbar_wait(bar_s, 0);
-        tc_fence_after();
-        // pass 1: row max
-        float m = -INFINITY;
-#pragma unroll
-        for (int j = 0; j < MAX_PREFIX; ++j) m = fmaxf(m, s_pre[j]);
-        // keys [kmin,kmax) are visible
-        const int kmin = p.pack ? (row_valid ? pseq * T : 0) : 0;
-        const int kmax = p.pack ? (row_valid ? kmin + T : 0) : (p.causal ? min(HW, qpos + 1) : HW);
-        for (int c = 0; c < kvrows; c += 32) {
-            // tcgen05.ld is warp-collective: a chunk is skipped only when no lane of the warp needs it
-            if (__all_sync(0xffffffffu, c + 32 <= kmin || c >= kmax)) continue;
-            uint32_t rr[32];
-            tmem_ld_32x32(trow + c, rr);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i)
-                if (c + i >= kmin && c + i < kmax) m = fmaxf(m, __uint_as_float(rr[i]));
-        }
-        const float msc = (m == -INFINITY) ? 0.f : m * p.scale_log2;
-        // pass 2: p = exp2(s*scale*log2e - m*scale*log2e), written as bf16 to the swizzled P tile, half by half
-        float l = 0.f;
-        float p_pre[MAX_PREFIX];
-#pragma unroll
-        for (int j = 0; j < MAX_PREFIX; ++j) {
-            p_pre[j] = (s_pre[j] == -INFINITY) ? 0.f : ex2f(s_pre[j] * p.scale_log2 - msc);
-            l += p_pre[j];
-            p_pre[j] = bf16_round(p_pre[j]);
-        }
-        for (int half = 0; half < p.nkt; ++half) {
-            if (half == 1) mbar_wait(bar_pv0, 0);  // P buffer free again
-#pragma unroll 1
-            for (int c32 = 0; c32 < 4; ++c32) {
-                const int c = half * 128 + c32 * 32;
-                uint32_t pk[16];
-                if (__all_sync(0xffffffffu, c + 32 <= kmin || c >= kmax)) {  // masked for the whole warp: zeros (PV sums over all keys)
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) pk[i] = 0u;
-                } else {
-                    uint32_t rr[32];
-                    tmem_ld_32x32(trow + c, rr);
-                    tmem_ld_wait();
-#pragma unroll
-                    for (int i = 0; i < 32; i += 2) {
-                        const bool v0 = c + i >= kmin && c + i < kmax, v1 = c + i + 1 >= kmin && c + i + 1 < kmax;
-                        float e0 = v0 ? ex2f(__uint_as_float(rr[i]) * p.scale_log2 - msc) : 0.f;
-                        float e1 = v1 ? ex2f(__uint_as_float(rr[i + 1]) * p.scale_log2 - msc) : 0.f;
-                        l += e0 + e1;
-                        pk[i >> 1] = pack_bf16x2(e0, e1);
-                    }
-                }
-                // 32 keys = 4 x 16B chunks into chunk-region (c32>>1), columns (c32&1)*32 ..
-                uint8_t* pb = smem + SP + (c32 >> 1) * 16384;
-#pragma unroll
-                for (int v4 = 0; v4 < 4; ++v4) {
-                    const int col = (c32 & 1) * 32 + v4 * 8;
-                    *reinterpret_cast<uint4*>(pb + sw128_off(r, col)) =
-                        make_uint4(pk[v4 * 4], pk[v4 * 4 + 1], pk[v4 * 4 + 2], pk[v4 * 4 + 3]);
-                }
-            }
-            tc_fence_before();
-            fence_proxy_async_smem();
-            mbar_arrive(half == 0 ? bar_p0 : bar_p1);
-        }
-        // epilogue
-        mbar_wait(bar_o, 0);
-        tc_fence_after();
-        uint32_t o0[32], o1[32];
-        tmem_ld_32x32(trow, o0);
-        tmem_ld_32x32(trow + 32, o1);
-        tmem_ld_wait();
-        float o[64];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) o[i] = __uint_as_float(o0[i]), o[32 + i] = __uint_as_float(o1[i]);
-#pragma unroll
-        for (int j = 0; j < MAX_PREFIX; ++j) {
-            if (j < prefix && p_pre[j] != 0.f) {
-                const uint4* vp = reinterpret_cast<const uint4*>(p.qkv + (seq_row0 + j) * 3 * D + 2 * D + h * 64);
-#pragma unroll
-                for (int c = 0; c < 8; ++c) {
-                    const uint4 w = __ldg(vp + c);
-                    o[c * 8 + 0] += p_pre[j] * bf16_lo(w.x), o[c * 8 + 1] += p_pre[j] * bf16_hi(w.x);
-                    o[c * 8 + 2] += p_pre[j] * bf16_lo(w.y), o[c * 8 + 3] += p_pre[j] * bf16_hi(w.y);
-                    o[c * 8 + 4] += p_pre[j] * bf16_lo(w.z), o[c * 8 + 5] += p_pre[j] * bf16_hi(w.z);
-                    o[c * 8 + 6] += p_pre[j] * bf16_lo(w.w), o[c * 8 + 7] += p_pre[j] * bf16_hi(w.w);
-                }
-            }
-        }
-        if (row_valid) {
-            const float inv = 1.f / l;
-            __nv_bfloat16* op = p.out + (seq_row0 + qtok) * D + h * 64;
-#pragma unroll
-            for (int c = 0; c < 8; ++c) {
-                uint4 w;
-                w.x = pack_bf16x2(o[c * 8] * inv, o[c * 8 + 1] * inv), w.y = pack_bf16x2(o[c * 8 + 2] * inv, o[c * 8 + 3] * inv);
-                w.z = pack_bf16x2(o[c * 8 + 4] * inv, o[c * 8 + 5] * inv), w.w = pack_bf16x2(o[c * 8 + 6] * inv, o[c * 8 + 7] * inv);
-                *reinterpret_cast<uint4*>(op + c * 8) = w;
-            }
-            if (p.lse) {
-                if (p.pack) p.lse[((long)(b + pseq) * p.H + h) * T + (r - pseq * T)] = m * p.scale + logf(l);
-                else p.lse[((long)b * p.H + h) * T + qtok] = m * p.scale + logf(l);
-            }
-        }
-        tc_fence_before();
-    } else {
-        // ---------------- warp 5: prefix query rows (only the qt==0 CTA), CUDA cores over the smem K/V tiles
+        // ---------------- warp 8: prefix query rows (only the qt==0 CTA), CUDA cores over the smem K/V tiles
         if (qt == 0 && prefix > 0) {
             mbar_wait(bar_qk, 0);
             mbar_wait(bar_v, 0);
@@ -345,349 +309,8 @@ __global__ void __launch_bounds__(ATT_THREADS, 2) attn_fwd_kernel(const __grid_c
             }
         }
     }
-
-    __syncthreads();
-    if (warp == 0) {
-        tc_fence_after();
-        tmem_dealloc(tmem, 256);
-    }
 }
 
-
-// ------------------------------------------------------------------------------------------------------------
-// Variant with TWO row threads per query row (opt-in: VTP_ATTN_FWD8=1).  The one-thread-per-row kernel above is
-// latency-bound (profiles/ncu_attn_r1b_before_cls_fix.md: 16 % warps active, 24 % issue slots, 5 % tensor pipe): its 4
-// row warps per CTA walk 256 score columns serially.  Here 8 row warps share the 128 TMEM lanes pairwise (warps w and
-// w+4 own the same lane quarter, as in attn_bwd_kernel): both compute the full-row max (the cheap pass), then each
-// exponentiates HALF of the columns, writes its half of P and later normalises half of the 64 output dims.  With two
-// 128-key halves the second P half goes into the Q|K0 region, which is dead once S is complete and the cls warp has
-// finished its score pass (bar_kfree) — so both halves are produced concurrently and smem stays at 2 CTAs/SM.  The row
-// sums are exchanged once, after the last MMA, through the then-dead P buffer.
-static constexpr int ATT8_THREADS = 320;  // warp 0: TMA + MMA; warps 1-8: row warps; warp 9: prefix (cls) query rows
-
-__global__ void __launch_bounds__(ATT8_THREADS, 2) attn_fwd8_kernel(const __grid_constant__ CUtensorMap tm, const AttnDev p) {
-    extern __shared__ __align__(1024) uint8_t smem[];
-    if (smem_u32(smem) & 1023) __trap();
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SBAR);
-    uint64_t* bar_qk = bars + 0;     // Q,K landed
-    uint64_t* bar_v = bars + 1;      // V landed
-    uint64_t* bar_s = bars + 2;      // S complete in TMEM
-    uint64_t* bar_p0 = bars + 3;     // P half 0 written
-    uint64_t* bar_p1 = bars + 4;     // P half 1 written (nkt == 2)
-    uint64_t* bar_o = bars + 5;      // O complete
-    uint64_t* bar_kfree = bars + 6;  // cls warp has finished reading the K tiles
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int qt = blockIdx.x, h = blockIdx.y, b = p.pack ? blockIdx.z * p.pack : blockIdx.z;
-    const int D = p.D, T = p.T, prefix = p.prefix, HW = p.HW, nkt = p.nkt;
-    const long seq_row0 = (long)b * T;
-    const int kvrows = 128 * nkt;
-
-    if (threadIdx.x == 0) {
-        tma_prefetch_desc(&tm);
-        mbar_init(bar_qk, 1), mbar_init(bar_v, 1), mbar_init(bar_s, 1), mbar_init(bar_p0, nkt == 2 ? 128 : 256);
-        mbar_init(bar_p1, 128), mbar_init(bar_o, 1), mbar_init(bar_kfree, 1);
-        fence_barrier_init();
-    }
-    if (warp == 0) {
-        tmem_alloc(tmem_slot, 256);
-        tmem_relinquish();
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-
-    if (warp == 0) {
-        if (lane == 0) {
-            const int row_q = (int)seq_row0 + prefix + 128 * qt;
-            const int row_k = (int)seq_row0 + prefix;
-            mbar_expect_tx(bar_qk, 16384 + 16384 * nkt);
-            tma_load_2d(smem + SQ, &tm, bar_qk, h * 64, row_q);
-            for (int i = 0; i < nkt; ++i) tma_load_2d(smem + SK + i * 16384, &tm, bar_qk, D + h * 64, row_k + 128 * i);
-            mbar_expect_tx(bar_v, 16384 * nkt);
-            for (int i = 0; i < nkt; ++i) tma_load_2d(smem + SV + i * 16384, &tm, bar_v, 2 * D + h * 64, row_k + 128 * i);
-            mbar_wait(bar_qk, 0);
-            tc_fence_after();
-            const uint32_t idesc_s = umma_idesc_bf16(128, kvrows, 0, 0);
-            const uint32_t qa = smem_u32(smem + SQ), ka = smem_u32(smem + SK);
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-                umma_bf16_ss(tmem, umma_desc_sw128(qa + j * 32, 0, 1024), umma_desc_sw128(ka + j * 32, 0, 1024), idesc_s,
-                             j > 0);
-            umma_commit(bar_s);
-            const uint32_t idesc_o = umma_idesc_bf16(128, 64, 0, 1);  // B (= V) is MN-major
-            const uint32_t va = smem_u32(smem + SV);
-            mbar_wait(bar_v, 0);
-            for (int half = 0; half < nkt; ++half) {
-                mbar_wait(half == 0 ? bar_p0 : bar_p1, 0);
-                tc_fence_after();
-                const uint32_t pa = smem_u32(smem + (half == 0 ? SP : SQ));  // half 1 lives in the dead Q|K0 region
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    const uint64_t ad = umma_desc_sw128(pa + (j >> 2) * 16384 + (j & 3) * 32, 0, 1024);
-                    const uint64_t bd = umma_desc_sw128(va + half * 16384 + j * 2048, 8192, 1024);
-                    umma_bf16_ss(tmem, ad, bd, idesc_o, (half > 0 || j > 0) ? 1u : 0u);
-                }
-            }
-            umma_commit(bar_o);
-        }
-    } else if (warp <= 8) {
-        const int set = (warp - 1) >> 2;  // 0: first half of the columns / output dims, 1: second half
-        const int q4 = warp & 3;          // TMEM lane quarter this warp may access (== warp id % 4)
-        const int r = q4 * 32 + lane;
-        const int qpos = 128 * qt + r;
-        const int qtok = prefix + qpos;
-        const int pseq = p.pack ? r / T : 0;
-        const bool row_valid = p.pack ? (pseq < p.pack && b + pseq < p.B) : (qpos < HW);
-        const uint32_t trow = tmem + (uint32_t(q4 * 32) << 16);
-
-        float s_pre[MAX_PREFIX];
-        mbar_wait(bar_qk, 0);
-        if (prefix > 0) {
-            float qf[64];
-#pragma unroll
-            for (int c = 0; c < 8; ++c) {
-                const uint4 w = *reinterpret_cast<const uint4*>(smem + SQ + sw128_off(r, c * 8));
-                qf[c * 8 + 0] = bf16_lo(w.x), qf[c * 8 + 1] = bf16_hi(w.x), qf[c * 8 + 2] = bf16_lo(w.y);
-                qf[c * 8 + 3] = bf16_hi(w.y), qf[c * 8 + 4] = bf16_lo(w.z), qf[c * 8 + 5] = bf16_hi(w.z);
-                qf[c * 8 + 6] = bf16_lo(w.w), qf[c * 8 + 7] = bf16_hi(w.w);
-            }
-#pragma unroll
-            for (int j = 0; j < MAX_PREFIX; ++j) {
-                s_pre[j] = -INFINITY;
-                if (j < prefix) {
-                    const uint4* kp = reinterpret_cast<const uint4*>(p.qkv + (seq_row0 + j) * 3 * D + D + h * 64);
-                    float acc = 0.f;
-#pragma unroll
-                    for (int c = 0; c < 8; ++c) {
-                        const uint4 w = __ldg(kp + c);
-                        acc += qf[c * 8 + 0] * bf16_lo(w.x) + qf[c * 8 + 1] * bf16_hi(w.x) + qf[c * 8 + 2] * bf16_lo(w.y) +
-                               qf[c * 8 + 3] * bf16_hi(w.y) + qf[c * 8 + 4] * bf16_lo(w.z) + qf[c * 8 + 5] * bf16_hi(w.z) +
-                               qf[c * 8 + 6] * bf16_lo(w.w) + qf[c * 8 + 7] * bf16_hi(w.w);
-                    }
-                    if (!p.causal || j <= qtok) s_pre[j] = acc;
-                }
-            }
-        } else {
-#pragma unroll
-            for (int j = 0; j < MAX_PREFIX; ++j) s_pre[j] = -INFINITY;
-        }
-
-        mbar_wait(bar_s, 0);
-        tc_fence_after();
-        // pass 1 (both threads of a row, redundantly): row max over all visible keys
-        float m = -INFINITY;
-#pragma unroll
-        for (int j = 0; j < MAX_PREFIX; ++j) m = fmaxf(m, s_pre[j]);
-        const int kmin = p.pack ? (row_valid ? pseq * T : 0) : 0;
-        const int kmax = p.pack ? (row_valid ? kmin + T : 0) : (p.causal ? min(HW, qpos + 1) : HW);
-        for (int c = 0; c < kvrows; c += 32) {
-            if (__all_sync(0xffffffffu, c + 32 <= kmin || c >= kmax)) continue;
-            uint32_t rr[32];
-            tmem_ld_32x32(trow + c, rr);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i)
-                if (c + i >= kmin && c + i < kmax) m = fmaxf(m, __uint_as_float(rr[i]));
-        }
-        // Every row thread has now (a) read its Q row for the prefix scores and (b) finished reading ALL score columns.
-        // Both matter before anyone moves on: the second P half overwrites the Q tile, and the first P·V MMA overwrites
-        // score columns [0,64) with O while a slower partner thread could still be scanning them for its maximum.
-        tc_fence_before();
-        asm volatile("bar.sync 2, 256;" ::: "memory");
-        tc_fence_after();
-        const float msc = (m == -INFINITY) ? 0.f : m * p.scale_log2;
-        float l = 0.f;
-        float p_pre[MAX_PREFIX];
-#pragma unroll
-        for (int j = 0; j < MAX_PREFIX; ++j) {
-            p_pre[j] = (s_pre[j] == -INFINITY) ? 0.f : ex2f(s_pre[j] * p.scale_log2 - msc);
-            if (set == 0) l += p_pre[j];        // the prefix key columns are counted once per row
-            p_pre[j] = bf16_round(p_pre[j]);
-        }
-        // pass 2: my half of the columns.  nkt == 2: key half `set` (its own P buffer); nkt == 1: 64 of the 128 keys
-        const bool second_buf = (nkt == 2 && set == 1);
-        if (second_buf && qt == 0 && prefix > 0) mbar_wait(bar_kfree, 0);  // K0 tile is about to be overwritten
-        uint8_t* pbase = smem + (second_buf ? SQ : SP);
-        const int nchunk = (nkt == 2) ? 4 : 2;
-#pragma unroll 1
-        for (int i = 0; i < nchunk; ++i) {
-            const int c32 = (nkt == 2) ? i : 2 * set + i;          // 32-key chunk within the 128-key P tile
-            const int c = ((nkt == 2) ? set * 128 : 0) + c32 * 32;  // score column
-            uint32_t pk[16];
-            if (__all_sync(0xffffffffu, c + 32 <= kmin || c >= kmax)) {
-#pragma unroll
-                for (int k = 0; k < 16; ++k) pk[k] = 0u;
-            } else {
-                uint32_t rr[32];
-                tmem_ld_32x32(trow + c, rr);
-                tmem_ld_wait();
-#pragma unroll
-                for (int k = 0; k < 32; k += 2) {
-                    const bool v0 = c + k >= kmin && c + k < kmax, v1 = c + k + 1 >= kmin && c + k + 1 < kmax;
-                    const float e0 = v0 ? ex2f(__uint_as_float(rr[k]) * p.scale_log2 - msc) : 0.f;
-                    const float e1 = v1 ? ex2f(__uint_as_float(rr[k + 1]) * p.scale_log2 - msc) : 0.f;
-                    l += e0 + e1;
-                    pk[k >> 1] = pack_bf16x2(e0, e1);
-                }
-            }
-            uint8_t* pb = pbase + (c32 >> 1) * 16384;
-#pragma unroll
-            for (int v4 = 0; v4 < 4; ++v4) {
-                const int col = (c32 & 1) * 32 + v4 * 8;
-                *reinterpret_cast<uint4*>(pb + sw128_off(r, col)) =
-                    make_uint4(pk[v4 * 4], pk[v4 * 4 + 1], pk[v4 * 4 + 2], pk[v4 * 4 + 3]);
-            }
-        }
-        tc_fence_before();
-        fence_proxy_async_smem();
-        mbar_arrive(second_buf ? bar_p1 : bar_p0);
-
-        // epilogue: wait for O, exchange the partial row sums through the (now dead) P buffer, normalise 32 dims each
-        mbar_wait(bar_o, 0);
-        tc_fence_after();
-        float* xs = reinterpret_cast<float*>(smem + SP);
-        xs[set * 128 + r] = l;
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        l = xs[r] + xs[128 + r];
-        uint32_t o0[32];
-        tmem_ld_32x32(trow + 32 * set, o0);
-        tmem_ld_wait();
-        float o[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) o[i] = __uint_as_float(o0[i]);
-#pragma unroll
-        for (int j = 0; j < MAX_PREFIX; ++j) {
-            if (j < prefix && p_pre[j] != 0.f) {
-                const uint4* vp = reinterpret_cast<const uint4*>(p.qkv + (seq_row0 + j) * 3 * D + 2 * D + h * 64 + 32 * set);
-#pragma unroll
-                for (int c = 0; c < 4; ++c) {
-                    const uint4 w = __ldg(vp + c);
-                    o[c * 8 + 0] += p_pre[j] * bf16_lo(w.x), o[c * 8 + 1] += p_pre[j] * bf16_hi(w.x);
-                    o[c * 8 + 2] += p_pre[j] * bf16_lo(w.y), o[c * 8 + 3] += p_pre[j] * bf16_hi(w.y);
-                    o[c * 8 + 4] += p_pre[j] * bf16_lo(w.z), o[c * 8 + 5] += p_pre[j] * bf16_hi(w.z);
-                    o[c * 8 + 6] += p_pre[j] * bf16_lo(w.w), o[c * 8 + 7] += p_pre[j] * bf16_hi(w.w);
-                }
-            }
-        }
-        if (row_valid) {
-            const float inv = 1.f / l;
-            __nv_bfloat16* op = p.out + (seq_row0 + qtok) * D + h * 64 + 32 * set;
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-                uint4 w;
-                w.x = pack_bf16x2(o[c * 8] * inv, o[c * 8 + 1] * inv), w.y = pack_bf16x2(o[c * 8 + 2] * inv, o[c * 8 + 3] * inv);
-                w.z = pack_bf16x2(o[c * 8 + 4] * inv, o[c * 8 + 5] * inv), w.w = pack_bf16x2(o[c * 8 + 6] * inv, o[c * 8 + 7] * inv);
-                *reinterpret_cast<uint4*>(op + c * 8) = w;
-            }
-            if (p.lse && set == 0) {
-                if (p.pack) p.lse[((long)(b + pseq) * p.H + h) * T + (r - pseq * T)] = m * p.scale + logf(l);
-                else p.lse[((long)b * p.H + h) * T + qtok] = m * p.scale + logf(l);
-            }
-        }
-        tc_fence_before();
-    } else {
-        // ---------------- warp 9: prefix query rows (only the qt == 0 CTA), CUDA cores over the smem K/V tiles
-        if (qt == 0 && prefix > 0) {
-            mbar_wait(bar_qk, 0);
-            mbar_wait(bar_v, 0);
-            for (int j = 0; j < prefix; ++j) {
-                float qf[64];
-                {
-                    const uint4* qp = reinterpret_cast<const uint4*>(p.qkv + (seq_row0 + j) * 3 * D + h * 64);
-#pragma unroll
-                    for (int c = 0; c < 8; ++c) {
-                        const uint4 w = __ldg(qp + c);
-                        qf[c * 8 + 0] = bf16_lo(w.x), qf[c * 8 + 1] = bf16_hi(w.x), qf[c * 8 + 2] = bf16_lo(w.y);
-                        qf[c * 8 + 3] = bf16_hi(w.y), qf[c * 8 + 4] = bf16_lo(w.z), qf[c * 8 + 5] = bf16_hi(w.z);
-                        qf[c * 8 + 6] = bf16_lo(w.w), qf[c * 8 + 7] = bf16_hi(w.w);
-                    }
-                }
-                auto dot_row = [&](const uint4* kp, bool from_smem, int row) {
-                    float acc = 0.f;
-#pragma unroll
-                    for (int c = 0; c < 8; ++c) {
-                        const uint4 w = from_smem ? *reinterpret_cast<const uint4*>(smem + SK + sw128_off(row, c * 8))
-                                                  : __ldg(kp + c);
-                        acc += qf[c * 8 + 0] * bf16_lo(w.x) + qf[c * 8 + 1] * bf16_hi(w.x) + qf[c * 8 + 2] * bf16_lo(w.y) +
-                               qf[c * 8 + 3] * bf16_hi(w.y) + qf[c * 8 + 4] * bf16_lo(w.z) + qf[c * 8 + 5] * bf16_hi(w.z) +
-                               qf[c * 8 + 6] * bf16_lo(w.w) + qf[c * 8 + 7] * bf16_hi(w.w);
-                    }
-                    return acc;
-                };
-                float sp[MAX_PREFIX], s[8];
-                float m = -INFINITY;
-#pragma unroll
-                for (int t = 0; t < MAX_PREFIX; ++t) {
-                    sp[t] = -INFINITY;
-                    if (t < prefix && (!p.causal || t <= j))
-                        sp[t] = dot_row(reinterpret_cast<const uint4*>(p.qkv + (seq_row0 + t) * 3 * D + D + h * 64), false, 0);
-                    m = fmaxf(m, sp[t]);
-                }
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    const int kk = lane + 32 * i;
-                    s[i] = -INFINITY;
-                    if (kk < HW && kk < kvrows && (!p.causal || prefix + kk <= j)) s[i] = dot_row(nullptr, true, kk);
-                    m = fmaxf(m, s[i]);
-                }
-                __syncwarp();
-                if (j == prefix - 1 && lane == 0) mbar_arrive(bar_kfree);  // last read of the K tiles is behind us
-                m = warp_max(m);
-                const float msc = m * p.scale_log2;
-                float l = 0.f;
-                __nv_bfloat16* pcls = reinterpret_cast<__nv_bfloat16*>(smem + SPCLS);
-                __syncwarp();
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    const float e = (s[i] == -INFINITY) ? 0.f : ex2f(s[i] * p.scale_log2 - msc);
-                    l += e;
-                    pcls[lane + 32 * i] = __float2bfloat16_rn(e);
-                }
-                l = warp_sum(l);
-                __syncwarp();
-                float a0 = 0.f, a1 = 0.f, c0 = 0.f, c1 = 0.f;
-#pragma unroll
-                for (int t = 0; t < MAX_PREFIX; ++t) {
-                    if (t < prefix && sp[t] != -INFINITY) {
-                        const float pe = ex2f(sp[t] * p.scale_log2 - msc);
-                        l += pe;
-                        const uint32_t w = __ldg(reinterpret_cast<const uint32_t*>(p.qkv + (seq_row0 + t) * 3 * D + 2 * D + h * 64) + lane);
-                        a0 += bf16_round(pe) * bf16_lo(w), a1 += bf16_round(pe) * bf16_hi(w);
-                    }
-                }
-                const int kend = min(HW, kvrows);
-                for (int k8 = 0; k8 < kend; k8 += 8) {
-                    const uint4 pw = *reinterpret_cast<const uint4*>(pcls + k8);
-                    const uint32_t pr[4] = {pw.x, pw.y, pw.z, pw.w};
-#pragma unroll
-                    for (int u = 0; u < 8; ++u) {
-                        const float pk = (u & 1) ? bf16_hi(pr[u >> 1]) : bf16_lo(pr[u >> 1]);
-                        const uint32_t w = *reinterpret_cast<const uint32_t*>(smem + SV + sw128_off(k8 + u, 2 * lane));
-                        if (u & 1) c0 += pk * bf16_lo(w), c1 += pk * bf16_hi(w);
-                        else a0 += pk * bf16_lo(w), a1 += pk * bf16_hi(w);
-                    }
-                }
-                a0 += c0, a1 += c1;
-                const float inv = 1.f / l;
-                *reinterpret_cast<uint32_t*>(p.out + (seq_row0 + j) * D + h * 64 + 2 * lane) = pack_bf16x2(a0 * inv, a1 * inv);
-                if (p.lse && lane == 0) p.lse[((long)b * p.H + h) * T + j] = m * p.scale + logf(l);
-            }
-        }
-    }
-
-    __syncthreads();
-    if (warp == 0) {
-        tc_fence_after();
-        tmem_dealloc(tmem, 256);
-    }
-}
-
-}  // namespace vtp
-
-namespace vtp {
 
 // ------------------------------------------------------------------------------------------------------------
 // fp32 attention (accuracy mode): CUDA cores, one CTA per (head, image), K/V tiles in padded smem, one warp per
@@ -774,20 +397,13 @@ extern "C" int vtp_attention_fwd(const void* qkv, void* out, float* lse, int B, 
     if (rc) return rc;
     static bool configured = false;
     if (!configured) {
-        VTP_CUDA(cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
-        VTP_CUDA(cudaFuncSetAttribute(attn_fwd8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
+        VTP_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
+        VTP_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
         configured = true;
     }
     dim3 grid(p.pack ? 1 : ceil_div(HW, 128), H, p.pack ? ceil_div(B, p.pack) : B);
-    // persistent ping-pong kernel (attention_pipe.cu) for 128 < HW <= 256: default since its round-2 hardware validation
-    // (x1.11 and bit-identical); VTP_ATTN_FWD_PIPE=0 selects the one-tile-per-CTA kernel below
-    const char* vp = getenv("VTP_ATTN_FWD_PIPE");
-    if (!(vp && vp[0] == '0') && !p.pack && !causal && p.nkt == 2 && HW % 8 == 0) return attn_fwd_pipe_launch(tm, p, (cudaStream_t)st);
-    const char* v8 = getenv("VTP_ATTN_FWD8");  // opt-in: two row threads per query row (see attn_fwd8_kernel)
-    if (v8 && v8[0] == '1')
-        attn_fwd8_kernel<<<grid, ATT8_THREADS, ATT_SMEM, (cudaStream_t)st>>>(tm, p);
-    else
-        attn_fwd_kernel<<<grid, ATT_THREADS, ATT_SMEM, (cudaStream_t)st>>>(tm, p);
+    if (p.nkt == 2) attn_fwd_kernel<2><<<grid, ATT_THREADS, ATT_SMEM, (cudaStream_t)st>>>(tm, p);
+    else attn_fwd_kernel<1><<<grid, ATT_THREADS, ATT_SMEM, (cudaStream_t)st>>>(tm, p);
     VTP_LAUNCH_CHECK();
     return VTP_OK;
 }

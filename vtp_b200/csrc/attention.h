@@ -1,4 +1,4 @@
-// vtp_b200 — argument block shared by the attention forward kernels (attention.cu, attention_pipe.cu).
+// vtp_b200 — argument block of the attention forward kernel (attention.cu).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -17,8 +17,5 @@ struct AttnDev {
     float scale_log2;                         // scale * log2(e)
     float scale;
 };
-
-// persistent ping-pong forward for 128 < HW <= 256 (attention_pipe.cu); default for those shapes, VTP_ATTN_FWD_PIPE=0 opts out
-int attn_fwd_pipe_launch(const CUtensorMap& tm, const AttnDev& p, cudaStream_t st);
 
 }  // namespace vtp

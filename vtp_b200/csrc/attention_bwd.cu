@@ -1,18 +1,14 @@
-// vtp_b200 — fused self-attention BACKWARD for short sequences (T = prefix + HW, prefix <= 1, HW <= 256) on tcgen05.
+// vtp_b200 — fused self-attention BACKWARD for short sequences (T = prefix + HW, prefix <= 1, HW <= 256) on wgmma.
 //
 // Gradient of layers/attention.py:110-126 (RoPE + SDPA) w.r.t. the packed pre-RoPE qkv projection output:
 //   P = exp(s·QKᵀ − lse)      dV = Pᵀ dO      dP = dO Vᵀ      dS = s · P ∘ (dP − δ),  δ_i = Σ_d dO_id O_id
 //   dQ = dS K                 dK = dSᵀ Q      then RoPEᵀ on dQ, dK (rotation is linear: layers/attention.py:12-23)
 //
-// One CTA per (head, image).  All five GEMMs run on tcgen05 with the operands exactly as TMA lands them (128-row x
-// 64-col bf16 tiles of Q, K, V out of the packed qkv buffer and of dO): the transposes are expressed through the UMMA
-// major-ness bits —  Pᵀ / dSᵀ are MN-major A operands read from the same swizzled smem tile that serves dS as a K-major
-// A operand for dQ; dO, Q, K are MN-major B operands.  Work is split in (key half kh, query tile t) steps:
-//   MMA1: S = Q_t K_khᵀ, dP = dO_t V_khᵀ   (TMEM cols 256..511)      -> 128 row-threads build P, dS (bf16, smem)
-//   MMA2: dV_kh += Pᵀ dO_t, dK_kh += dSᵀ Q_t (TMEM 0..127), dQ_t += dS K_kh (TMEM 128..255)
-// TMEM: dK|dV (128) + dQ_0|dQ_1 (128) + S|dP (256) = 512 columns.
-// The cls token (prefix) is handled on CUDA cores as in the forward kernel: as an extra key column by the row threads
-// (rank-1 updates + a warp-reduced column for dK_0/dV_0) and as an extra query row by a spare warp.
+// All five GEMMs run on wgmma with the operands exactly as TMA lands them (128-row x 64-col bf16 tiles of Q, K, V out of
+// the packed qkv buffer and of dO): the transposes are expressed through the wgmma transpose bits — Pᵀ / dSᵀ are MN-major
+// A operands read from the same swizzled smem tile that serves dS as a K-major A operand for dQ; dO, Q, K are MN-major B
+// operands.  The cls token (prefix) is handled on CUDA cores as in the forward kernel: as an extra key column by the row
+// threads (rank-1 updates + a column reduction for dK_0/dV_0) and as an extra query row by a spare warp.
 #include <stdlib.h>
 
 #include "host.h"
@@ -20,14 +16,11 @@
 
 namespace vtp {
 
-#ifndef VTP_ATTN_BWD_TSO_DEFAULT
-#define VTP_ATTN_BWD_TSO_DEFAULT 1  // TMA-store row epilogues of the FULL path (measured: 502.5 -> 450.0 us, same bits)
-#endif
-static constexpr int AB_THREADS = 320;  // 8 row warps (2 per scheduler) + TMA/MMA warp + cls warp
+static constexpr int AB_THREADS = 384;  // 2 consumer warpgroups + warpgroup 2 (warp 8: TMA, cls query row)
 static constexpr int BQ = 0, BK_ = 32768, BV = 65536, BDO = 98304, BP = 131072, BDS = 163840, BX = 196608;
 // extras after BX: p0[264] | ds0[264] | dk0[64] | dv0[64] | pcol[2][128] | dscol[2][128] | barriers
 static constexpr int X_P0 = 0, X_DS0 = 1056, X_DK0 = 2112, X_DV0 = 2368, X_PCOL = 2624, X_DSCOL = 3648, X_BAR = 4672;
-static constexpr int AB_SMEM = BX + X_BAR + 128;
+static constexpr int AB_SMEM = BX + X_BAR + 128 + 1024;  // + alignment slack
 
 struct AttnBwdDev {
     const __nv_bfloat16* qkv;   // [B*T][3D] post-RoPE q,k ; v
@@ -42,8 +35,6 @@ struct AttnBwdDev {
     // packed mode (T <= 64): `pack` whole sequences share the 128-row tile, their prefix tokens (`rprefix` per sequence)
     // are ordinary rows / key columns (prefix == 0 above) and P, dS are masked block-diagonally
     int pack, rprefix;
-    int tso;       // FULL only: last-key-half dK/dV rows and the dQ rows leave through shared memory + one TMA store per warp
-    int prefetch;  // row threads pull their O rows (delta = dO.O) and lse towards L2/L1 before the tile loads are waited for
 };
 
 __device__ __forceinline__ float ex2f(float x) {  // ex2.approx.ftz: no denormal slow path (exp2f() costs 4 extra instr)
@@ -94,36 +85,32 @@ __device__ __forceinline__ void rope_bwd64(float (&g)[64], const __nv_bfloat16* 
     }
 }
 
-// bf16 row (64 values) of a warp's 32-row slab -> the warp's 4 KB staging tile (128-byte swizzle, as the tensor map expects),
-// then ONE TMA store of the [32 rows x 64 columns] box: replaces eight scattered 16-byte global stores per thread whose
-// drain stalled the row threads at the end of every CTA (profiles/ncu_attn_r2b warp-state samples)
-__device__ __forceinline__ void stage_store_row64(const CUtensorMap* tmap, uint8_t* warp_stage, int lane, const float (&f)[64], int x,
-                                                  int y) {
-    uint8_t* ob = warp_stage + lane * 128;
+// RoPEᵀ on the 16 dims of a row that a thread of the quad holds in an m64n64 accumulator fragment: g[2 jn + c] is dim
+// 8 jn + 2 c4 + c, so dims d and d + 32 (jn and jn + 4) sit in the same thread
+__device__ __forceinline__ void rope_bwd_frag(float (&g)[16], const __nv_bfloat16* sin_row, const __nv_bfloat16* cos_row, int c4) {
 #pragma unroll
-    for (int c = 0; c < 8; ++c) {
-        uint4 w;
-        w.x = pack_bf16x2(f[c * 8], f[c * 8 + 1]), w.y = pack_bf16x2(f[c * 8 + 2], f[c * 8 + 3]);
-        w.z = pack_bf16x2(f[c * 8 + 4], f[c * 8 + 5]), w.w = pack_bf16x2(f[c * 8 + 6], f[c * 8 + 7]);
-        *reinterpret_cast<uint4*>(ob + ((c ^ (lane & 7)) << 4)) = w;
-    }
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0) {
-        tma_store_2d(tmap, warp_stage, x, y);
-        bulk_commit();
+    for (int jn = 0; jn < 4; ++jn) {
+        const int d = 8 * jn + 2 * c4;
+        const uint32_t s_lo = __ldg(reinterpret_cast<const uint32_t*>(sin_row + d));
+        const uint32_t s_hi = __ldg(reinterpret_cast<const uint32_t*>(sin_row + d + 32));
+        const uint32_t c_lo = __ldg(reinterpret_cast<const uint32_t*>(cos_row + d));
+        const uint32_t c_hi = __ldg(reinterpret_cast<const uint32_t*>(cos_row + d + 32));
+        const float sl[2] = {bf16_lo(s_lo), bf16_hi(s_lo)}, sh[2] = {bf16_lo(s_hi), bf16_hi(s_hi)};
+        const float cl[2] = {bf16_lo(c_lo), bf16_hi(c_lo)}, ch[2] = {bf16_lo(c_hi), bf16_hi(c_hi)};
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+            const float a = g[2 * jn + c], b = g[2 * (jn + 4) + c];
+            g[2 * jn + c] = a * cl[c] + b * sh[c];
+            g[2 * (jn + 4) + c] = b * ch[c] - a * sl[c];
+        }
     }
 }
 
-// FULL: HW == 256, no packing, no causal mask — every (query, key) pair of every step is valid, so the P / dS loop runs
-// without per-element predicates (ncu, profiles/ncu_attn_r2a.md: ~30 executed instructions per score element in the
-// generic loop, mostly mask predicates, selects and address arithmetic) and with hoisted swizzle offsets.
-template <bool FULL>
-__global__ void __launch_bounds__(AB_THREADS, 1)
-attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constant__ CUtensorMap tm_do,
-                const __grid_constant__ CUtensorMap tm_dq, const AttnBwdDev p) {
-    extern __shared__ __align__(1024) uint8_t smem[];
-    if (smem_u32(smem) & 1023) __trap();
+template <int NKT>
+__global__ void __launch_bounds__(AB_THREADS, 1) attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constant__ CUtensorMap tm_do,
+                                                 const AttnBwdDev p) {
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     float* p0 = reinterpret_cast<float*>(smem + BX + X_P0);
     float* ds0 = reinterpret_cast<float*>(smem + BX + X_DS0);
     float* dk0 = reinterpret_cast<float*>(smem + BX + X_DK0);
@@ -131,52 +118,241 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constan
     float* pcol = reinterpret_cast<float*>(smem + BX + X_PCOL);
     float* dscol = reinterpret_cast<float*>(smem + BX + X_DSCOL);
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + BX + X_BAR);
-    uint64_t* bar_ld = bars + 0;       // [2] tile loads
-    uint64_t* bar_sdp = bars + 2;      // S,dP in TMEM
-    uint64_t* bar_pds = bars + 3;      // P,dS in smem (128 arrivals), S/dP TMEM consumed
-    uint64_t* bar_mma2 = bars + 4;     // dV/dK/dQ MMAs of a step complete
-    uint64_t* bar_accfree = bars + 5;  // dK/dV accumulators drained by the epilogue (128 arrivals)
-    uint64_t* bar_cls = bars + 6;      // p0/ds0 rows written by the cls warp
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
+    uint64_t* bar_ld = bars + 0;   // [2] tile loads
+    uint64_t* bar_cls = bars + 2;  // p0/ds0 rows written by the cls warp
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int h = blockIdx.x, b = p.pack ? blockIdx.y * p.pack : blockIdx.y;
-    const int D = p.D, T = p.T, prefix = p.prefix, HW = p.HW, nkt = p.nkt;
+    const int D = p.D, T = p.T, prefix = p.prefix, HW = p.HW;
     const long row0 = (long)b * T;
-    const int nsteps = nkt * nkt;
+    const int nkt = NKT;
     const float lse_l2 = 1.4426950408889634f;
 
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&tm_qkv);
         tma_prefetch_desc(&tm_do);
-        if (FULL && p.tso) tma_prefetch_desc(&tm_dq);
-        mbar_init(&bar_ld[0], 1), mbar_init(&bar_ld[1], 1), mbar_init(bar_sdp, 1), mbar_init(bar_pds, 256);
-        mbar_init(bar_mma2, 1), mbar_init(bar_accfree, 256), mbar_init(bar_cls, 1);
+        mbar_init(&bar_ld[0], 1), mbar_init(&bar_ld[1], 1), mbar_init(bar_cls, 1);
         fence_barrier_init();
     }
     if (threadIdx.x < 128) dk0[threadIdx.x & 63] = 0.f, dv0[threadIdx.x & 63] = 0.f;
-    if (p.prefetch && !p.pack && warp < 8) {
-        // warp-state samples (profiles/ncu_attn_r2b): ~10 % of the row threads' time was the first-touch latency of their
-        // O rows (one 128-byte line per row and head, straight from HBM) at the start of every CTA
-        const int rr = (warp & 3) * 32 + lane, tt = warp >> 2;   // group g = warp >> 2 prefetches query tile g
-        if (tt < nkt && 128 * tt + rr < HW)
-            asm volatile("prefetch.global.L2 [%0];" ::"l"(p.o + (row0 + prefix + 128 * tt + rr) * D + h * 64));
-    }
-    if (warp == 8) {
-        tmem_alloc(tmem_slot, 512);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    // TMEM columns
-    const uint32_t C_DV = 0, C_DK = 64, C_DQ = 128 /* + 64*t */, C_S = 256, C_DP = 384;
 
-    if (warp == 8) {
+    if (warp < 8) {
+        setmaxnreg_inc<200>();  // 384 x 168 registers: + 256 x 32 here = - 128 x 64 in warpgroup 2
+        const int wg = warp >> 2, tw = threadIdx.x & 127, c4 = lane & 3;
+        const uint32_t aQ = smem_u32(smem + BQ), aK = smem_u32(smem + BK_), aV = smem_u32(smem + BV);
+        const uint32_t aDO = smem_u32(smem + BDO), aP = smem_u32(smem + BP), aDS = smem_u32(smem + BDS);
+        int rr[2], pseq[2], ptok[2];
+        bool pvalid[2];
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            rr[i] = 64 * wg + 16 * (tw >> 5) + (lane >> 2) + 8 * i;
+            // packed mode: row r = token (r % T) of sequence b + r / T; it sees the key columns of its own sequence only
+            pseq[i] = p.pack ? rr[i] / T : 0;
+            pvalid[i] = p.pack && pseq[i] < p.pack && b + pseq[i] < p.B;
+            ptok[i] = rr[i] - pseq[i] * T;
+        }
+        const __nv_bfloat16* kcls = p.qkv + row0 * 3 * D + D + h * 64;
+        const __nv_bfloat16* vcls = p.qkv + row0 * 3 * D + 2 * D + h * 64;
+        float lse_i[NKT][2], delta_i[NKT][2], ds_own[NKT][2];
+        float dv[32], dk[32], dq[NKT][32];
+        // quad-split 64-dim dot product of two bf16 rows (16 dims per thread of the quad), summed over the quad
+        auto dot_quad = [&](const uint8_t* tile, int row, const __nv_bfloat16* g) {
+            float acc = 0.f;
+#pragma unroll
+            for (int c = 0; c < 2; ++c) {
+                const uint4 a = *reinterpret_cast<const uint4*>(tile + sw_off(row, 16 * c4 + 8 * c));
+                const uint4 w = __ldg(reinterpret_cast<const uint4*>(g + 16 * c4 + 8 * c));
+                const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, ww[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+                for (int e = 0; e < 4; ++e) acc += bf16_lo(aw[e]) * bf16_lo(ww[e]) + bf16_hi(aw[e]) * bf16_hi(ww[e]);
+            }
+            acc += __shfl_xor_sync(0xffffffffu, acc, 1);
+            acc += __shfl_xor_sync(0xffffffffu, acc, 2);
+            return acc;
+        };
+
+#pragma unroll
+        for (int n = 0; n < NKT * NKT; ++n) {
+            const int kh = n / NKT, t = n % NKT;
+            if (kh == 0) {
+                // per-query-tile scalars (first visit of tile t): lse, delta = dO·O, and the cls-key column
+                mbar_wait(&bar_ld[t], 0);
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const int qi = 128 * t + rr[i];
+                    const bool qvalid = p.pack ? pvalid[i] : qi < HW;
+                    const long grow = row0 + prefix + qi;
+                    lse_i[t][i] = 0.f, delta_i[t][i] = 0.f, ds_own[t][i] = 0.f;
+                    float p0v = 0.f, ds0v = 0.f;
+                    if (__any_sync(0xffffffffu, qvalid)) {  // quads are uniform: the shuffles stay inside valid quads
+                        const float dl = dot_quad(smem + BDO + t * 16384, rr[i], p.o + (qvalid ? grow : row0) * D + h * 64);
+                        if (qvalid) {
+                            lse_i[t][i] = p.pack ? p.lse[((long)(b + pseq[i]) * p.H + h) * T + ptok[i]]
+                                                 : p.lse[((long)b * p.H + h) * T + prefix + qi];
+                            delta_i[t][i] = dl;
+                        }
+                        if (prefix > 0) {
+                            const float dp0 = dot_quad(smem + BDO + t * 16384, rr[i], vcls);
+                            const float s0 = dot_quad(smem + BQ + t * 16384, rr[i], kcls);
+                            if (qvalid) {
+                                p0v = ex2f(s0 * p.scale_log2 - lse_i[t][i] * lse_l2);
+                                ds0v = p.scale * p0v * (dp0 - dl);
+                            }
+                        }
+                    }
+                    ds_own[t][i] = ds0v;
+                    if (prefix > 0 && c4 == 0) pcol[t * 128 + rr[i]] = p0v, dscol[t * 128 + rr[i]] = ds0v;
+                }
+                if (prefix > 0) {
+                    // column reductions for the cls key: dV_0 += Σ_i p_i0 dO_i ; dK_0 += Σ_i ds_i0 q_i
+                    asm volatile("bar.sync 1, 256;" ::: "memory");
+                    if (threadIdx.x < 128) {
+                        const int d = threadIdx.x & 63;
+                        const bool isk = threadIdx.x >= 64;
+                        const uint8_t* tile = smem + (isk ? BQ : BDO) + t * 16384;
+                        const float* colv = (isk ? dscol : pcol) + t * 128;
+                        float acc = 0.f;
+                        for (int r = 0; r < 128; ++r)
+                            acc = fmaf(colv[r], __uint_as_float((uint32_t)*reinterpret_cast<const uint16_t*>(tile + sw_off(r, d)) << 16), acc);
+                        atomicAdd(isk ? &dk0[d] : &dv0[d], acc);
+                    }
+                }
+            }
+            if (n == 1 && NKT == 2) mbar_wait(&bar_ld[1], 0);
+            // the P / dS tiles are free once both warpgroups have finished the previous step's MMAs
+            asm volatile("bar.sync 1, 256;" ::: "memory");
+#pragma unroll
+            for (int c = 0; c < 2; ++c) {  // 64-key chunk c of key half kh
+                float s[32], dpr[32];
+                wgmma_fence();
+#pragma unroll
+                for (int j = 0; j < 4; ++j)
+                    wgmma_m64n64_ss<0, 0>(s, wgmma_desc_sw128(aQ + t * 16384 + wg * 8192 + j * 32, 0, 1024),
+                                          wgmma_desc_sw128(aK + kh * 16384 + c * 8192 + j * 32, 0, 1024), j > 0);
+#pragma unroll
+                for (int j = 0; j < 4; ++j)
+                    wgmma_m64n64_ss<0, 0>(dpr, wgmma_desc_sw128(aDO + t * 16384 + wg * 8192 + j * 32, 0, 1024),
+                                          wgmma_desc_sw128(aV + kh * 16384 + c * 8192 + j * 32, 0, 1024), j > 0);
+                wgmma_commit();
+                wgmma_wait<0>();
+                fence_regs(s);
+                fence_regs(dpr);
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const int qi = 128 * t + rr[i];
+                    const bool qvalid = p.pack ? pvalid[i] : qi < HW;
+                    const int kmin = p.pack ? pseq[i] * T : 0;
+                    const int kmax = p.pack ? kmin + T : (p.causal ? min(HW, qi + 1) : HW);
+                    const float lsc = lse_i[t][i] * lse_l2, dl = delta_i[t][i];
+#pragma unroll
+                    for (int jn = 0; jn < 8; ++jn) {
+                        const int key = 128 * kh + 64 * c + 8 * jn + 2 * c4;
+                        float pe[2], de[2];
+#pragma unroll
+                        for (int cc = 0; cc < 2; ++cc) {
+                            pe[cc] = 0.f, de[cc] = 0.f;
+                            if (qvalid && key + cc >= kmin && key + cc < kmax) {
+                                pe[cc] = ex2f(s[4 * jn + 2 * i + cc] * p.scale_log2 - lsc);
+                                de[cc] = p.scale * pe[cc] * (dpr[4 * jn + 2 * i + cc] - dl);
+                            }
+                        }
+                        const uint32_t off = c * 16384 + sw_off(rr[i], 8 * jn + 2 * c4);
+                        *reinterpret_cast<uint32_t*>(smem + BP + off) = pack_bf16x2(pe[0], pe[1]);
+                        *reinterpret_cast<uint32_t*>(smem + BDS + off) = pack_bf16x2(de[0], de[1]);
+                    }
+                }
+            }
+            fence_proxy_async_smem();
+            asm volatile("bar.sync 1, 256;" ::: "memory");
+            // P / dS tile: [128 q][128 keys] as 2 chunks of 64 keys.  As MN-major A (M = keys): chunk wg, K-step of 16
+            // queries = 2048 B, SBO = 1024 (8 queries).  As K-major A (M = queries): k-step 32 B inside a chunk, next chunk
+            // +16384, my 64 query rows +8192.
+            wgmma_fence();
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {  // reduction over 128 queries
+                const uint64_t bdo = wgmma_desc_sw128(aDO + t * 16384 + j * 2048, 8192, 1024);
+                const uint64_t bq = wgmma_desc_sw128(aQ + t * 16384 + j * 2048, 8192, 1024);
+                wgmma_m64n64_ss<1, 1>(dv, wgmma_desc_sw128(aP + wg * 16384 + j * 2048, 8192, 1024), bdo, (t > 0 || j > 0));
+                wgmma_m64n64_ss<1, 1>(dk, wgmma_desc_sw128(aDS + wg * 16384 + j * 2048, 8192, 1024), bq, (t > 0 || j > 0));
+            }
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {  // reduction over 128 keys
+                const uint64_t ads = wgmma_desc_sw128(aDS + (j >> 2) * 16384 + wg * 8192 + (j & 3) * 32, 0, 1024);
+                const uint64_t bk = wgmma_desc_sw128(aK + kh * 16384 + j * 2048, 8192, 1024);
+                wgmma_m64n64_ss<0, 1>(dq[t], ads, bk, (kh > 0 || j > 0));
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs(dv);
+            fence_regs(dk);
+            fence_regs(dq[t]);
+
+            if (t == NKT - 1) {
+                // ------------ epilogue of key half kh: my key rows kj = 128 kh + rr[i]; acc[4 jn + 2 i + c] = dim 8 jn + 2 c4 + c
+                if (prefix > 0) mbar_wait(bar_cls, 0);
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const int kj = 128 * kh + rr[i];
+                    if (!(p.pack ? pvalid[i] : kj < HW)) continue;
+                    float gv[16], gk[16];
+#pragma unroll
+                    for (int e = 0; e < 16; ++e) {
+                        const int jn = e >> 1, cc = e & 1;
+                        gv[e] = dv[4 * jn + 2 * i + cc], gk[e] = dk[4 * jn + 2 * i + cc];
+                    }
+                    if (prefix > 0) {
+                        const float pc = p0[kj], dc = ds0[kj];
+                        const __nv_bfloat16* docls = p.dout + row0 * D + h * 64;  // dO of the cls query
+                        const __nv_bfloat16* qc = p.qkv + row0 * 3 * D + h * 64;  // q of the cls query
+#pragma unroll
+                        for (int jn = 0; jn < 8; ++jn) {
+                            const uint32_t wd = __ldg(reinterpret_cast<const uint32_t*>(docls + 8 * jn + 2 * c4));
+                            const uint32_t wq = __ldg(reinterpret_cast<const uint32_t*>(qc + 8 * jn + 2 * c4));
+                            gv[2 * jn] += pc * bf16_lo(wd), gv[2 * jn + 1] += pc * bf16_hi(wd);
+                            gk[2 * jn] += dc * bf16_lo(wq), gk[2 * jn + 1] += dc * bf16_hi(wq);
+                        }
+                    }
+                    const int pos = p.pack ? ptok[i] - p.rprefix : kj;  // patch position (prefix tokens are not rotated)
+                    if (p.rope_sin && pos >= 0) rope_bwd_frag(gk, p.rope_sin + (long)pos * 64, p.rope_cos + (long)pos * 64, c4);
+                    __nv_bfloat16* drow = p.dqkv + (row0 + prefix + kj) * 3 * D + h * 64;
+#pragma unroll
+                    for (int jn = 0; jn < 8; ++jn) {
+                        *reinterpret_cast<uint32_t*>(drow + 2 * D + 8 * jn + 2 * c4) = pack_bf16x2(gv[2 * jn], gv[2 * jn + 1]);
+                        *reinterpret_cast<uint32_t*>(drow + D + 8 * jn + 2 * c4) = pack_bf16x2(gk[2 * jn], gk[2 * jn + 1]);
+                    }
+                }
+            }
+        }
+        // ------------ dQ epilogue of every query tile
+#pragma unroll
+        for (int t = 0; t < NKT; ++t) {
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const int qi = 128 * t + rr[i];
+                if (!(p.pack ? pvalid[i] : qi < HW)) continue;
+                float gq[16];
+#pragma unroll
+                for (int e = 0; e < 16; ++e) gq[e] = dq[t][4 * (e >> 1) + 2 * i + (e & 1)];
+                if (prefix > 0) {
+#pragma unroll
+                    for (int jn = 0; jn < 8; ++jn) {
+                        const uint32_t w = __ldg(reinterpret_cast<const uint32_t*>(kcls + 8 * jn + 2 * c4));
+                        gq[2 * jn] += ds_own[t][i] * bf16_lo(w), gq[2 * jn + 1] += ds_own[t][i] * bf16_hi(w);
+                    }
+                }
+                const int pos = p.pack ? ptok[i] - p.rprefix : qi;
+                if (p.rope_sin && pos >= 0) rope_bwd_frag(gq, p.rope_sin + (long)pos * 64, p.rope_cos + (long)pos * 64, c4);
+                __nv_bfloat16* drow = p.dqkv + (row0 + prefix + qi) * 3 * D + h * 64;
+#pragma unroll
+                for (int jn = 0; jn < 8; ++jn)
+                    *reinterpret_cast<uint32_t*>(drow + 8 * jn + 2 * c4) = pack_bf16x2(gq[2 * jn], gq[2 * jn + 1]);
+            }
+        }
+    } else if (setmaxnreg_dec<104>(), warp == 8) {
         if (lane == 0) {
             // ------------------------------------------------ TMA: tile i = rows [128i, 128i+128) of Q,K,V,dO
-            for (int i = 0; i < nkt; ++i) {
+            for (int i = 0; i < NKT; ++i) {
                 const int r = (int)row0 + prefix + 128 * i;
                 mbar_expect_tx(&bar_ld[i], 4 * 16384);
                 tma_load_2d(smem + BQ + i * 16384, &tm_qkv, &bar_ld[i], h * 64, r);
@@ -184,291 +360,9 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constan
                 tma_load_2d(smem + BV + i * 16384, &tm_qkv, &bar_ld[i], 2 * D + h * 64, r);
                 tma_load_2d(smem + BDO + i * 16384, &tm_do, &bar_ld[i], h * 64, r);
             }
-            const uint32_t id_nt = umma_idesc_bf16(128, 128, 0, 0);  // S, dP: A K-major, B K-major
-            const uint32_t id_tn = umma_idesc_bf16(128, 64, 1, 1);   // dV, dK: A MN-major (Pᵀ), B MN-major
-            const uint32_t id_nn = umma_idesc_bf16(128, 64, 0, 1);   // dQ: A K-major (dS), B MN-major (K)
-            const uint32_t aQ = smem_u32(smem + BQ), aK = smem_u32(smem + BK_), aV = smem_u32(smem + BV);
-            const uint32_t aDO = smem_u32(smem + BDO), aP = smem_u32(smem + BP), aDS = smem_u32(smem + BDS);
-            auto mma1 = [&](int kh, int t) {
-#pragma unroll
-                for (int j = 0; j < 4; ++j)
-                    umma_bf16_ss(tmem + C_S, umma_desc_sw128(aQ + t * 16384 + j * 32, 0, 1024),
-                                 umma_desc_sw128(aK + kh * 16384 + j * 32, 0, 1024), id_nt, j > 0);
-#pragma unroll
-                for (int j = 0; j < 4; ++j)
-                    umma_bf16_ss(tmem + C_DP, umma_desc_sw128(aDO + t * 16384 + j * 32, 0, 1024),
-                                 umma_desc_sw128(aV + kh * 16384 + j * 32, 0, 1024), id_nt, j > 0);
-                umma_commit(bar_sdp);
-            };
-            mbar_wait(&bar_ld[0], 0);
-            tc_fence_after();
-            mma1(0, 0);
-            bool ld1_waited = false;
-            for (int n = 0; n < nsteps; ++n) {
-                const int kh = n / nkt, t = n % nkt;
-                mbar_wait(bar_pds, n & 1);
-                tc_fence_after();
-                if (n + 1 < nsteps) {
-                    if (!ld1_waited) mbar_wait(&bar_ld[1], 0), ld1_waited = true;
-                    mma1((n + 1) / nkt, (n + 1) % nkt);
-                }
-                if (kh > 0 && t == 0) {  // dK/dV accumulators of the previous key half must be drained
-                    mbar_wait(bar_accfree, (kh - 1) & 1);
-                    tc_fence_after();
-                }
-                // P / dS tile: [128 q][128 keys] as 2 chunks of 64 keys.  As MN-major A (M = keys): LBO = chunk
-                // stride 16384, SBO = 1024 (8 queries), K-step of 16 queries = 2048 B.  As K-major A (M = queries):
-                // k-step 32 B inside a chunk, next chunk +16384.
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {  // reduction over 128 queries
-                    const uint64_t bdo = umma_desc_sw128(aDO + t * 16384 + j * 2048, 8192, 1024);
-                    const uint64_t bq = umma_desc_sw128(aQ + t * 16384 + j * 2048, 8192, 1024);
-                    umma_bf16_ss(tmem + C_DV, umma_desc_sw128(aP + j * 2048, 16384, 1024), bdo, id_tn, (t > 0 || j > 0));
-                    umma_bf16_ss(tmem + C_DK, umma_desc_sw128(aDS + j * 2048, 16384, 1024), bq, id_tn, (t > 0 || j > 0));
-                }
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {  // reduction over 128 keys
-                    const uint64_t ads = umma_desc_sw128(aDS + (j >> 2) * 16384 + (j & 3) * 32, 0, 1024);
-                    const uint64_t bk = umma_desc_sw128(aK + kh * 16384 + j * 2048, 8192, 1024);
-                    umma_bf16_ss(tmem + C_DQ + 64 * t, ads, bk, id_nn, (kh > 0 || j > 0));
-                }
-                umma_commit(bar_mma2);
-            }
         }
-    } else if (warp < 8) {
-        // ---------------------------------------------------- row threads: 2 groups x 128 (one TMEM lane each).
-        // group g builds the P/dS columns of 64-key chunk g in every step, owns query tile g (cls-key column terms,
-        // dQ epilogue) and one of the two accumulators in the key-half epilogue (g=0: dV, g=1: dK).
-        const int g = warp >> 2, q4 = warp & 3;
-        const int r = q4 * 32 + lane;
-        const uint32_t trow = tmem + (uint32_t(q4 * 32) << 16);
-        // packed mode: row r = token (r % T) of sequence b + r / T; it sees the key columns of its own sequence only
-        const int pseq = p.pack ? r / T : 0;
-        const bool pvalid = p.pack && pseq < p.pack && b + pseq < p.B;
-        const int ptok = r - pseq * T;
-        const int my_tile = (nkt == 2) ? g : 0;
-        const bool owns_tile = (nkt == 2) || (g == 0);
-        float lse_i[2], delta_i[2];
-        float ds_own = 0.f;
-        const __nv_bfloat16* kcls = p.qkv + row0 * 3 * D + D + h * 64;
-        const __nv_bfloat16* vcls = p.qkv + row0 * 3 * D + 2 * D + h * 64;
-
-        for (int n = 0; n < nsteps; ++n) {
-            const int kh = n / nkt, t = n % nkt;
-            const int qi = 128 * t + r;  // patch index of my query row in this step
-            const bool qvalid = p.pack ? pvalid : qi < HW;
-            if (kh == 0) {
-                // per-query-tile scalars (first visit of tile t): lse, delta = dO·O; the owner group also does the
-                // cls-key column
-                mbar_wait(&bar_ld[t], 0);
-                lse_i[t] = 0.f, delta_i[t] = 0.f;
-                const bool mine = owns_tile && t == my_tile && prefix > 0;
-                float p0v = 0.f, ds0v = 0.f;
-                if (qvalid) {
-                    const long grow = row0 + prefix + qi;
-                    lse_i[t] = p.pack ? p.lse[((long)(b + pseq) * p.H + h) * T + ptok] : p.lse[((long)b * p.H + h) * T + prefix + qi];
-                    float dof[64], tmpf[64];
-                    load_row64(smem + BDO + t * 16384, r, dof);
-                    load_grow64(p.o + grow * D + h * 64, tmpf);
-                    float dl = 0.f;
-#pragma unroll
-                    for (int d = 0; d < 64; ++d) dl += dof[d] * tmpf[d];
-                    delta_i[t] = dl;
-                    if (mine) {
-                        load_grow64(vcls, tmpf);
-                        float dp0 = 0.f;
-#pragma unroll
-                        for (int d = 0; d < 64; ++d) dp0 += dof[d] * tmpf[d];
-                        load_row64(smem + BQ + t * 16384, r, dof);  // q row
-                        load_grow64(kcls, tmpf);
-                        float s0 = 0.f;
-#pragma unroll
-                        for (int d = 0; d < 64; ++d) s0 += dof[d] * tmpf[d];
-                        p0v = ex2f(s0 * p.scale_log2 - lse_i[t] * lse_l2);
-                        ds0v = p.scale * p0v * (dp0 - dl);
-                    }
-                }
-                if (mine) {
-                    // column reductions for the cls key: dV_0 += Σ_i p_i0 dO_i ; dK_0 += Σ_i ds_i0 q_i.  The per-row
-                    // scalars go through smem, then thread (which, d) walks the 128 rows of the dO / Q tile.
-                    ds_own = ds0v;
-                    pcol[g * 128 + r] = p0v, dscol[g * 128 + r] = ds0v;
-                    asm volatile("bar.sync %0, 128;" ::"r"(1 + g) : "memory");
-                    const int d = r & 63;
-                    const bool isk = r >= 64;
-                    const uint8_t* tile = smem + (isk ? BQ : BDO) + t * 16384;
-                    const float* colv = (isk ? dscol : pcol) + g * 128;
-                    // element (row i, dim d) of a swizzled 128-byte-row tile: row i = 8 a + k sits at a*1024 + k*128 +
-                    // (((d >> 3) ^ k) << 4) + 2 (d & 7): the eight k-offsets are loop invariant, a*1024 an immediate
-                    uint32_t ok[8];
-#pragma unroll
-                    for (int k = 0; k < 8; ++k) ok[k] = (uint32_t)(k * 128 + ((((d >> 3) ^ k) << 4) | ((d & 7) << 1)));
-                    float acc0 = 0.f, acc1 = 0.f;
-#pragma unroll
-                    for (int a = 0; a < 16; ++a) {
-                        const float4 c0 = *reinterpret_cast<const float4*>(colv + 8 * a);
-                        const float4 c1 = *reinterpret_cast<const float4*>(colv + 8 * a + 4);
-                        const float cv[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
-#pragma unroll
-                        for (int k = 0; k < 8; ++k) {
-                            const uint32_t e = *reinterpret_cast<const uint16_t*>(tile + a * 1024 + ok[k]);
-                            if (k & 1) acc1 = fmaf(cv[k], __uint_as_float(e << 16), acc1);
-                            else acc0 = fmaf(cv[k], __uint_as_float(e << 16), acc0);
-                        }
-                    }
-                    atomicAdd(isk ? &dk0[d] : &dv0[d], acc0 + acc1);
-                }
-            }
-            mbar_wait(bar_sdp, n & 1);
-            tc_fence_after();
-            if (n > 0) mbar_wait(bar_mma2, (n - 1) & 1);  // P/dS smem tiles free again
-            const float lsc = lse_i[t] * lse_l2, dl = delta_i[t];
-            if constexpr (FULL) {
-                const float sl2 = p.scale_log2, sc = p.scale, dls = dl * p.scale;
-                uint8_t* pb_ = smem + BP + g * 16384 + r * 128;   // my row of 64-key chunk g of the P / dS tiles
-                uint8_t* db_ = smem + BDS + g * 16384 + r * 128;
-#pragma unroll
-                for (int cc = 0; cc < 2; ++cc) {
-                    const int c32 = 2 * g + cc;
-                    uint32_t rs[32], rd[32];
-                    tmem_ld_32x32(trow + C_S + c32 * 32, rs);
-                    tmem_ld_32x32(trow + C_DP + c32 * 32, rd);
-                    tmem_ld_wait();
-                    uint32_t pk[16], dk[16];
-#pragma unroll
-                    for (int i = 0; i < 32; i += 2) {
-                        const float pa = ex2f(fmaf(__uint_as_float(rs[i]), sl2, -lsc));
-                        const float pb = ex2f(fmaf(__uint_as_float(rs[i + 1]), sl2, -lsc));
-                        const float da = pa * fmaf(__uint_as_float(rd[i]), sc, -dls);       // s P (dP - delta)
-                        const float db = pb * fmaf(__uint_as_float(rd[i + 1]), sc, -dls);
-                        pk[i >> 1] = pack_bf16x2(pa, pb);
-                        dk[i >> 1] = pack_bf16x2(da, db);
-                    }
-#pragma unroll
-                    for (int v4 = 0; v4 < 4; ++v4) {
-                        const uint32_t off = (uint32_t)(((cc * 4 + v4) ^ (r & 7)) << 4);
-                        *reinterpret_cast<uint4*>(pb_ + off) = make_uint4(pk[v4 * 4], pk[v4 * 4 + 1], pk[v4 * 4 + 2], pk[v4 * 4 + 3]);
-                        *reinterpret_cast<uint4*>(db_ + off) = make_uint4(dk[v4 * 4], dk[v4 * 4 + 1], dk[v4 * 4 + 2], dk[v4 * 4 + 3]);
-                    }
-                }
-            } else {
-            const int kmin = p.pack ? pseq * T : 0;
-            const int kmax = p.pack ? kmin + T : (p.causal ? min(HW, qi + 1) : HW);
-#pragma unroll 1
-            for (int cc = 0; cc < 2; ++cc) {
-                const int c32 = 2 * g + cc;
-                uint32_t rs[32], rd[32];
-                tmem_ld_32x32(trow + C_S + c32 * 32, rs);
-                tmem_ld_32x32(trow + C_DP + c32 * 32, rd);
-                tmem_ld_wait();
-                uint32_t pk[16], dk[16];
-                const int kbase = 128 * kh + c32 * 32;
-#pragma unroll
-                for (int i = 0; i < 32; i += 2) {
-                    float pa = 0.f, pb = 0.f, da = 0.f, db = 0.f;
-                    if (qvalid && kbase + i >= kmin && kbase + i < kmax) {
-                        pa = ex2f(__uint_as_float(rs[i]) * p.scale_log2 - lsc);
-                        da = p.scale * pa * (__uint_as_float(rd[i]) - dl);
-                    }
-                    if (qvalid && kbase + i + 1 >= kmin && kbase + i + 1 < kmax) {
-                        pb = ex2f(__uint_as_float(rs[i + 1]) * p.scale_log2 - lsc);
-                        db = p.scale * pb * (__uint_as_float(rd[i + 1]) - dl);
-                    }
-                    pk[i >> 1] = pack_bf16x2(pa, pb);
-                    dk[i >> 1] = pack_bf16x2(da, db);
-                }
-                uint8_t* pb_ = smem + BP + g * 16384;   // 64-key chunk g of the P / dS tiles
-                uint8_t* db_ = smem + BDS + g * 16384;
-#pragma unroll
-                for (int v4 = 0; v4 < 4; ++v4) {
-                    const uint32_t off = sw_off(r, cc * 32 + v4 * 8);
-                    *reinterpret_cast<uint4*>(pb_ + off) = make_uint4(pk[v4 * 4], pk[v4 * 4 + 1], pk[v4 * 4 + 2], pk[v4 * 4 + 3]);
-                    *reinterpret_cast<uint4*>(db_ + off) = make_uint4(dk[v4 * 4], dk[v4 * 4 + 1], dk[v4 * 4 + 2], dk[v4 * 4 + 3]);
-                }
-            }
-            }
-            tc_fence_before();
-            fence_proxy_async_smem();
-            mbar_arrive(bar_pds);
-
-            if (t == nkt - 1) {
-                // ------------ epilogue of key half kh: I own key row kj = 128*kh + r; group 0 -> dV, group 1 -> dK
-                mbar_wait(bar_mma2, n & 1);
-                tc_fence_after();
-                const int kj = 128 * kh + r;
-                // last key half: the P / dS tiles are idle (their last MMAs have completed) and serve as store staging
-                const bool tso = FULL && p.tso && kh == nkt - 1;
-                uint32_t a0[32], a1[32];
-                float gq[64];
-                if (prefix > 0) mbar_wait(bar_cls, 0);
-                tmem_ld_32x32(trow + (g == 0 ? C_DV : C_DK), a0);
-                tmem_ld_32x32(trow + (g == 0 ? C_DV : C_DK) + 32, a1);
-                tmem_ld_wait();
-#pragma unroll
-                for (int i = 0; i < 32; ++i) gq[i] = __uint_as_float(a0[i]), gq[32 + i] = __uint_as_float(a1[i]);
-                tc_fence_before();
-                mbar_arrive(bar_accfree);
-                if (p.pack ? pvalid : kj < HW) {
-                    if (g == 0) {
-                        if (prefix > 0) {
-                            float f[64];
-                            load_grow64(p.dout + row0 * D + h * 64, f);  // dO of the cls query
-                            const float pc = p0[kj];
-#pragma unroll
-                            for (int d = 0; d < 64; ++d) gq[d] += pc * f[d];
-                        }
-                        if (tso)
-                            stage_store_row64(&tm_dq, smem + BP + q4 * 4096, lane, gq, 2 * D + h * 64,
-                                              (int)(row0 + prefix) + 128 * kh + q4 * 32);
-                        else store_row64(p.dqkv + (row0 + prefix + kj) * 3 * D + 2 * D + h * 64, gq);
-                    } else {
-                        if (prefix > 0) {
-                            float f[64];
-                            load_grow64(p.qkv + row0 * 3 * D + h * 64, f);  // q of the cls query
-                            const float dc = ds0[kj];
-#pragma unroll
-                            for (int d = 0; d < 64; ++d) gq[d] += dc * f[d];
-                        }
-                        const int pos = p.pack ? ptok - p.rprefix : kj;  // patch position (prefix tokens are not rotated)
-                        if (p.rope_sin && pos >= 0) rope_bwd64(gq, p.rope_sin + (long)pos * 64, p.rope_cos + (long)pos * 64);
-                        if (tso)
-                            stage_store_row64(&tm_dq, smem + BP + 16384 + q4 * 4096, lane, gq, D + h * 64,
-                                              (int)(row0 + prefix) + 128 * kh + q4 * 32);
-                        else store_row64(p.dqkv + (row0 + prefix + kj) * 3 * D + D + h * 64, gq);
-                    }
-                }
-            }
-        }
-        // ------------ dQ epilogue of my query tile (all steps done; last bar_mma2 phase already observed above)
-        if (owns_tile) {
-            const int t = my_tile;
-            const int qi = 128 * t + r;
-            uint32_t a0[32], a1[32];
-            tmem_ld_32x32(trow + C_DQ + 64 * t, a0);
-            tmem_ld_32x32(trow + C_DQ + 64 * t + 32, a1);
-            tmem_ld_wait();
-            if (p.pack ? pvalid : qi < HW) {
-                float gq[64];
-#pragma unroll
-                for (int i = 0; i < 32; ++i) gq[i] = __uint_as_float(a0[i]), gq[32 + i] = __uint_as_float(a1[i]);
-                if (prefix > 0) {
-                    float f[64];
-                    load_grow64(kcls, f);
-#pragma unroll
-                    for (int d = 0; d < 64; ++d) gq[d] += ds_own * f[d];
-                }
-                const int pos = p.pack ? ptok - p.rprefix : qi;
-                if (p.rope_sin && pos >= 0) rope_bwd64(gq, p.rope_sin + (long)pos * 64, p.rope_cos + (long)pos * 64);
-                if (FULL && p.tso)
-                    stage_store_row64(&tm_dq, smem + BDS + g * 16384 + q4 * 4096, lane, gq, h * 64,
-                                      (int)(row0 + prefix) + 128 * t + q4 * 32);
-                else store_row64(p.dqkv + (row0 + prefix + qi) * 3 * D + h * 64, gq);
-            }
-        }
-        if (FULL && p.tso && lane == 0) bulk_wait0();  // my warp's row stores have left shared memory and are complete
-        tc_fence_before();
-    } else {
-        // ---------------------------------------------------- warp 9: the cls query row (prefix == 1)
+        __syncwarp();
+        // ---------------------------------------------------- warp 8: the cls query row (prefix == 1)
         if (prefix > 0) {
             for (int i = 0; i < nkt; ++i) mbar_wait(&bar_ld[i], 0);
             float q0[64], do0[64];
@@ -531,7 +425,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constan
     }
 
     __syncthreads();
-    if (warp == 9 && prefix > 0) {
+    if (warp == 8 && prefix > 0) {
         // dV_0 = Σ_i p_i0 dO_i (+ p_00 dO_0) ;  dK_0 = Σ_i ds_i0 q_i (+ ds_00 q_0)   — cls key row, no RoPE
         const float p00 = p0[260], ds00 = ds0[260];
         const uint32_t wdo = __ldg(reinterpret_cast<const uint32_t*>(p.dout + row0 * D + h * 64) + lane);
@@ -541,11 +435,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constan
         *reinterpret_cast<uint32_t*>(p.dqkv + row0 * 3 * D + 2 * D + h * 64 + 2 * lane) = pack_bf16x2(v0, v1);
         *reinterpret_cast<uint32_t*>(p.dqkv + row0 * 3 * D + D + h * 64 + 2 * lane) = pack_bf16x2(k0, k1);
     }
-    if (warp == 8) {
-        tc_fence_after();
-        tmem_dealloc(tmem, 512);
-    }
 }
+
 
 }  // namespace vtp
 
@@ -570,22 +461,11 @@ extern "C" int vtp_attention_bwd(const void* qkv, const void* o, const void* dou
     p.nkt = HW > 128 ? 2 : 1;
     p.scale = 0.125f, p.scale_log2 = 0.125f * 1.4426950408889634f;
     p.pack = 0, p.rprefix = prefix;
-    p.prefetch = getenv("VTP_ATTN_BWD_NO_PREFETCH") == nullptr;
-    {
-        const char* ts = getenv("VTP_ATTN_BWD_TSO");
-        p.tso = ts ? ts[0] != '0' : VTP_ATTN_BWD_TSO_DEFAULT;
-    }
     if (!causal && T <= 64 && B > 1 && getenv("VTP_ATTN_NO_PACK") == nullptr) {
         p.pack = 128 / T;
         p.prefix = 0, p.HW = T, p.nkt = 1;
     }
-    CUtensorMap tq, td, tdq;
-    {   // dqkv [B*T][3D]: 32-row x 64-column boxes (one warp's rows of one head's dq / dk / dv)
-        uint64_t dims[2] = {(uint64_t)3 * D, (uint64_t)B * T}, strides[1] = {(uint64_t)3 * D * 2};
-        uint32_t box[2] = {64, 32};
-        int rc = make_tmap_bf16(&tdq, dqkv, 2, dims, strides, box);
-        if (rc) return rc;
-    }
+    CUtensorMap tq, td;
     {
         uint64_t dims[2] = {(uint64_t)3 * D, (uint64_t)B * T}, strides[1] = {(uint64_t)3 * D * 2};
         uint32_t box[2] = {64, 128};
@@ -600,15 +480,13 @@ extern "C" int vtp_attention_bwd(const void* qkv, const void* o, const void* dou
     }
     static bool configured = false;
     if (!configured) {
-        VTP_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, AB_SMEM));
-        VTP_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, AB_SMEM));
+        VTP_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, AB_SMEM));
+        VTP_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, AB_SMEM));
         configured = true;
     }
     const dim3 grid(H, p.pack ? ceil_div(B, p.pack) : B);
-    if (p.HW == 256 && !p.pack && !p.causal && getenv("VTP_ATTN_BWD_GENERIC") == nullptr)
-        attn_bwd_kernel<true><<<grid, AB_THREADS, AB_SMEM, (cudaStream_t)st>>>(tq, td, tdq, p);
-    else
-        attn_bwd_kernel<false><<<grid, AB_THREADS, AB_SMEM, (cudaStream_t)st>>>(tq, td, tdq, p);
+    if (p.nkt == 2) attn_bwd_kernel<2><<<grid, AB_THREADS, AB_SMEM, (cudaStream_t)st>>>(tq, td, p);
+    else attn_bwd_kernel<1><<<grid, AB_THREADS, AB_SMEM, (cudaStream_t)st>>>(tq, td, p);
     VTP_LAUNCH_CHECK();
     return VTP_OK;
 }

@@ -29,8 +29,8 @@ __device__ __forceinline__ void ld4<__nv_bfloat16>(const __nv_bfloat16* p, float
 // ------------------------------------------------------------------------------------------------ norm backward
 // g[m,:] += dx[m,:] where dx is the input-gradient of RMSNorm / LayerNorm given dy (bf16) ; dw += Σ dy∘xhat ; db += Σ dy
 // One warp per row, 8 rows per warp-iteration strip; per-block column partials -> fp32 atomics.
-// Occupancy: ncu (profiles/ncu_hbm_r2.md) showed the 512-thread / 124-register version at ONE block per SM (16 warps, 25 %
-// occupancy, 64 % of the copy bandwidth).  256-thread blocks capped at 80 registers run three per SM; D <= 384 gets its own
+// Occupancy: a 512-thread / 124-register version fits ONE block per SM (16 warps); 256-thread blocks capped at 80
+// registers run three per SM; D <= 384 gets its own
 // MAXV = 3 instantiation (36 column accumulators instead of 48) and the row values are re-derived from x, dy after the
 // row reduction instead of being kept in a second register array.
 template <typename TX, int MAXV>
@@ -328,8 +328,8 @@ __global__ void adamw_kernel(float* __restrict__ p, float* __restrict__ g, float
     }
     // 4 parameters per thread per iteration (all buffers are 128-byte aligned and n % 4 == 0 by construction).
     // The two divisions and the square root per parameter use the hardware approximations (MUFU.RCP / MUFU.SQRT, <= 2 ulp):
-    // ncu (profiles/ncu_hbm_r2.md) showed 660 executed instructions per float4 with the IEEE sequences and their slow-path
-    // branches — 28 % of the copy bandwidth; the update is rounded to a bf16 compute copy anyway.
+    // the IEEE sequences with their slow-path branches cost hundreds of instructions per float4, and the update is rounded
+    // to a bf16 compute copy anyway.
     const float ibc1 = 1.f / bc1, ibc2 = 1.f / bc2;
     for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n4; i += (long)gridDim.x * blockDim.x) {
         float4 gi = reinterpret_cast<float4*>(g)[i];

@@ -15,7 +15,7 @@
 //   vtp_clip_grad             dM_i = dL/dS rows of the rank's images (row-softmax term + column-softmax term),
 //                             dM_t likewise for its captions
 // Because every rank holds the full Bg x Bg logits (2·Bg²·E FLOP — microseconds), the feature gradients need NO
-// backward collective: dI_local = dM_i · T_all, dT_local = dM_t · I_all (two tcgen05 GEMMs).  The only exchange on the
+// backward collective: dI_local = dM_i · T_all, dT_local = dM_t · I_all (two wgmma GEMMs).  The only exchange on the
 // contrastive path is the forward gather, as north_star prescribes.
 #include "host.h"
 #include "ptx.cuh"

@@ -473,9 +473,8 @@ extern "C" int vtp_l2norm_fwd(const void* x, int x_dtype, void* y, int y_dtype, 
 }
 
 // ------------------------------------------------------------------------------------------------ SwiGLU gate / RoPE
-// Stand-alone (full-occupancy) versions of the two heaviest GEMM epilogues.  Measured on B200 (M = 131 584, D = 384):
-// fused SwiGLU epilogue 843-971 us vs plain GEMM 355 us + this kernel ~125 us; fused RoPE 436 us vs 216 + ~60 us — the
-// 8 epilogue warps of the GEMM are instruction/latency bound at K = 384, a 64-warp/SM elementwise pass is not.
+// Stand-alone (full-occupancy) versions of the two heaviest GEMM epilogues: at K = 384 the GEMM's 8 epilogue warps are
+// instruction / latency bound on the RoPE arithmetic, a 64-warp/SM elementwise pass is not.
 namespace vtp {
 // pre bf16 [M][2Hs] (8-interleaved x1|x2) -> hid bf16 [M][Hs] = round(round(silu(x1)) * x2)   (layers/ffn.py:77-81)
 __global__ void swiglu_fwd_kernel(const __nv_bfloat16* __restrict__ pre, __nv_bfloat16* __restrict__ hid, long M, int Hs) {

@@ -1,12 +1,13 @@
-// vtp_b200 — persistent, warp-specialised tcgen05 GEMM for sm_100a.
+// vtp_b200 — persistent, warp-specialised wgmma GEMM for sm_90a.
 //
-//   out[M,N] = epilogue( A[M,K] · B[N,K]ᵀ )      bf16 operands, fp32 accumulators in TMEM
+//   out[M,N] = epilogue( A[M,K] · B[N,K]ᵀ )      bf16 operands, fp32 accumulators
 //
-// Roles (192 threads): warp 0 = TMA producer, warp 1 = UMMA issuer (+ TMEM alloc), warps 2..5 = epilogue
-// (TMEM -> registers -> fused epilogue -> global).  BM = 128 (UMMA M=128, cta_group::1), BN in {128, 256},
-// BK = 64 bf16 = one 128B swizzle span.  The accumulator is double buffered in TMEM (2 x BN columns) so the
-// epilogue of tile i overlaps the MMAs of tile i+1.  Operands may be K-major or MN-major (UMMA major bits), so
-// forward (NT), dgrad (NN) and wgrad (TN) all run through this one kernel; wgrad uses split-K + fp32 atomics.
+// Roles (384 threads): warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 = consumers.  BM = 128 (each consumer
+// warpgroup issues m64 wgmma for its 64 rows), BN in {64, 128}, BK = 64 bf16 = one 128B swizzle span, a STAGES-deep
+// TMA / mbarrier ring.  Operands may be K-major or MN-major (wgmma transpose bits), so forward (NT), dgrad (NN) and wgrad
+// (TN) all run through this one kernel; wgrad uses split-K + fp32 atomics.  After the mainloop the accumulators go
+// through a padded fp32 tile in shared memory, from which the eight consumer warps run the epilogue with one output row
+// per lane (32-row slabs); the producer meanwhile already streams the next tile's operands.
 //
 // Fused epilogues (all optional): +bias, bf16 rounding point, GELU, SwiGLU gate (8-interleaved w1|w2), axial
 // RoPE on q/k (bf16 arithmetic exactly as layers/attention.py:12-23,70-89), +residual, row remap (cls-token
@@ -21,16 +22,7 @@ namespace vtp {
 static constexpr int BM = 128;
 static constexpr int BK = 64;
 static constexpr int A_BYTES = BM * BK * 2;
-static constexpr int BRES_KB = 9;                    // resident k-blocks of the B-resident conv form (3 x 3 taps x 64 channels)
-static constexpr int HALO_W = 16, HALO_H = 18;       // halo block of the BRES == 2 form: 18 rows of 16 pixels (tile 16 x 8)
-static constexpr int HALO_BYTES = HALO_W * HALO_H * BK * 2;
-#ifndef VTP_CONV_HALO_DEFAULT
-#define VTP_CONV_HALO_DEFAULT 1  // two-ring halo form for the other conv shapes with tiles <= 128 wide (measured: VGG per step 31.1 -> 29.1 ms)
-#endif
-#ifndef VTP_CONV_BRES_DEFAULT
-#define VTP_CONV_BRES_DEFAULT 2  // measured (profiles/r2_conv_halo.md): conv1_2 603 -> 357 (1) -> 205 us (2); 0 = off
-#endif
-static constexpr int NUM_THREADS = 320;  // TMA warp + MMA warp + 8 epilogue warps
+static constexpr int NUM_THREADS = 384;  // producer warpgroup + 2 consumer (MMA + epilogue) warpgroups
 
 struct GemmDev {
     int M, N, K;
@@ -54,16 +46,14 @@ struct GemmDev {
     int conv_C, conv_H, conv_W, conv_TW, conv_TH, conv_tiles_h, conv_tiles_w, conv_B;
     const __nv_bfloat16* mask_pos;  // optional: out *= (mask_pos[row][col] > 0)   (ReLU backward in the dgrad epilogue)
     int ldm;
-    int dbg;  // DIAG bits: 1 no global stores, 2 no tmem ld, 4 no epilogue work, 8 no MMA issue
 };
 
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f)); }
 
 // ---------------------------------------------------------------------------------------------------- epilogue
-// 8 epilogue warps (2 per SM sub-partition: with one warp per scheduler every TMEM/shared/global latency of the
-// epilogue was exposed and small-K GEMMs ran at 15 % of tensor peak).  Warp w owns TMEM lane quarter (w & 3) and the
-// 64-column units of parity (w >> 2).  A unit is processed in two phases:
-//   A (row owner: lane = TMEM lane = output row)  TMEM -> registers, +bias, rounding point, activation / RoPE
+// 8 epilogue warps (the consumer warps).  Warp w owns row quarter (w & 3) of the tile and the 64-column units of
+// parity (w >> 2).  A unit is processed in two phases:
+//   A (row owner: lane = output row)  accumulator tile -> registers, +bias, rounding point, activation / RoPE
 //   B (cooperative)  the slab goes, 32 columns at a time, through a per-warp XOR-swizzled fp32 staging tile (4 KB) so
 //     that every global access is a contiguous 128-byte line per quarter-warp: residual read (prefetched into registers
 //     before the accumulator is even waited for), dtype conversion, store / red.add / PixelShuffle scatter.
@@ -136,7 +126,6 @@ __device__ __forceinline__ void store_bf16(const GemmDev& p, const uint8_t* stg,
         const int R = 4 * it + (lane >> 3);
         const long orow = orow8[it];
         if (orow < 0 || !col_ok) continue;
-        if (p.dbg & 1) continue;
         uint4 w = *reinterpret_cast<const uint4*>(stg + stgb_off(R, cidx));
         if (has_resid && which == 0) {
             const uint4 rb = *reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(p.resid) + orow * p.ldr + ocol0 + c8);
@@ -170,7 +159,6 @@ __device__ __forceinline__ void store_half(const GemmDev& p, const float* stg, i
         const int grow = grow0 + R;
         const long orow = orow8[it];
         if (orow < 0 || !col_ok) continue;
-        if (p.dbg & 1) continue;
         float4 v = *reinterpret_cast<const float4*>(stg + stg_off(R, cidx));
         if (which == 1) {
             uint2 w;
@@ -361,25 +349,27 @@ __device__ __forceinline__ void epilogue_unit(const GemmDev& p, float* stg, int 
 // The recurring shapes of the training step (qkv / proj / fc1 / fc2 forward, every dgrad) need only bias, a bf16
 // rounding point, an optional residual of the output's own dtype and a store.  The generic epilogue above spends
 // ~550 instructions per 64-column unit (address math, feature branches, staging read-back), misses the instruction
-// cache and waits on its bias loads: short-K GEMMs ran at a third of what the mainloop sustains (profiles/
-// ncu_gemm_fc1_r1b.md).  This path: lane == accumulator row; one 128-byte output row piece per lane is written into a
+// cache and waits on its bias loads, which leaves short-K GEMMs epilogue-bound.  This path: lane == accumulator row; one 128-byte output row piece per lane is written into a
 // 4 KB SWIZZLE_128B staging tile and leaves through ONE TMA store (clipped at the M / N tails by the tensor map);
 // bias comes from a 256-byte per-warp shared tile (broadcast reads), the residual is fetched into registers one chunk
-// ahead, before the accumulator is waited for.
+// ahead.
 //   FAST: 1 bf16 out, 2 bf16 out + bf16 residual, 3 fp32 out, 4 fp32 out + fp32 residual, 5 bf16 out masked by
 //   (mask_pos > 0) (ReLU backward of the LPIPS dgrads).   ACT: NONE | RELU.
 // Implicit-conv GEMMs (tile = conv_TH x conv_TW pixel patch of one image) store through a 4-D NHWC tensor map: the warp's
 // 32 rows are 32 / conv_TW image rows of conv_TW pixels.
-// hand the accumulator buffer back to the MMA issuer: with cta_group::2 the issuer lives in the leader CTA (rank 0)
-template <bool G2>
-__device__ __forceinline__ void arrive_tempty(uint64_t* bar) {
-    if (G2) mbar_arrive_cluster(mapa_u32(bar, 0));
-    else mbar_arrive(bar);
+// 32 consecutive fp32 accumulator columns of this lane's row (the tile is padded: conflict-free 16-byte reads)
+__device__ __forceinline__ void acc_ld32(const float* arow, uint32_t (&r)[32]) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+        const float4 v = *reinterpret_cast<const float4*>(arow + 4 * i);
+        r[4 * i] = __float_as_uint(v.x), r[4 * i + 1] = __float_as_uint(v.y), r[4 * i + 2] = __float_as_uint(v.z),
+        r[4 * i + 3] = __float_as_uint(v.w);
+    }
 }
 
 // Tile index t = work_id, work_id + stride, ... decomposed as t = (ks * num_m + m) * num_n + n WITHOUT a division per tile: the
-// producer and the MMA issuer are single threads, and three runtime integer divisions per tile (~150 dependent instructions)
-// sat directly on the operand-feed path of the short-K GEMMs (found on the implicit-conv form, profiles/r2_logs/lpips_layers*).
+// producer is a single thread, and three runtime integer divisions per tile (~150 dependent instructions)
+// would sit directly on the operand-feed path of the short-K GEMMs.
 struct TileIter {
     int n, m, ks;          // current tile
     int dn, dm, dks;       // decomposition of the stride
@@ -405,18 +395,16 @@ struct TileIter {
 // [16g, 16g+8) = x1, [16g+8, 16g+16) = x2) stores them as the pre-activation through tmO2 and writes their 32 + 32 hidden
 // values  round(round(silu(x1)) * x2)  (layers/ffn.py:77-81 under autocast) into a second 32 x 128-byte staging tile that
 // leaves through ONE TMA store of the [M, Hs] hidden tensor (tmO).
-template <int BN, int FAST, bool G2>
+template <int BN, int FAST>
 __device__ __forceinline__ void fast_swiglu_tile(const GemmDev& p, const CUtensorMap* tmO, const CUtensorMap* tmO2, uint8_t* stg,
-                                                 uint8_t* stg2, float* bias_s, int lane, int q, int hsel, uint32_t taddr,
-                                                 int m_blk, int n0, uint64_t* tfull, uint32_t aph, uint64_t* tempty) {
+                                                 uint8_t* stg2, float* bias_s, int lane, int q, int hsel, const float* arow,
+                                                 int m_blk, int n0) {
     constexpr bool PRE = FAST == 6;
     constexpr int TCH = BN / 64;             // packed 64-column chunks per tile row (BN in {128, 256})
     const int m0 = m_blk * BM;
     const int N = p.N;
     const int c0 = 2 * hsel;                 // this warp's chunk pair (2 hsel, 2 hsel + 1) -> hidden columns [64 hsel, +64)
     const bool have = c0 < TCH && n0 + c0 * 64 < N;
-    mbar_wait(tfull, aph);
-    tc_fence_after();
     if (have) {
 #pragma unroll
         for (int j = 0; j < 2; ++j) {
@@ -424,19 +412,13 @@ __device__ __forceinline__ void fast_swiglu_tile(const GemmDev& p, const CUtenso
             const bool valid = col0 < N;     // warp-uniform (ragged last tile: N % 64 != 0 is clipped by the tensor maps)
             uint32_t r0[32], r1[32];
             if (valid) {
-                tmem_ld_32x32(taddr + (c0 + j) * 64, r0);
-                tmem_ld_32x32(taddr + (c0 + j) * 64 + 32, r1);
+                acc_ld32(arow + (c0 + j) * 64, r0);
+                acc_ld32(arow + (c0 + j) * 64 + 32, r1);
             }
             bias_s[lane] = (p.bias && col0 + lane < N) ? __ldg(p.bias + col0 + lane) : 0.f;
             bias_s[32 + lane] = (p.bias && col0 + 32 + lane < N) ? __ldg(p.bias + col0 + 32 + lane) : 0.f;
             if (lane == 0) bulk_wait_read0();   // earlier TMA stores of this warp have finished reading both staging tiles
             __syncwarp();
-            if (valid) tmem_ld_wait();
-            if (j == 1) {                       // accumulator fully in registers: hand the TMEM buffer back
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) arrive_tempty<G2>(tempty);
-            }
             uint32_t hw[16];                    // 32 hidden values of this chunk, packed
             uint32_t xs[32];                    // the chunk's ROUNDED values regrouped: [0,16) = x1 pairs, [16,32) = x2 pairs
 #pragma unroll
@@ -469,7 +451,7 @@ __device__ __forceinline__ void fast_swiglu_tile(const GemmDev& p, const CUtenso
 #pragma unroll
             for (int c = 0; c < 4; ++c)       // 32 hidden values = 64 bytes = chunks 4 j .. 4 j + 3 of the 128-byte hidden row
                 *reinterpret_cast<uint4*>(stg2 + stgb_off(lane, 4 * j + c)) = make_uint4(hw[4 * c], hw[4 * c + 1], hw[4 * c + 2], hw[4 * c + 3]);
-            if (PRE && valid && !(p.dbg & 1)) {
+            if (PRE && valid) {
                 fence_proxy_async_smem();
                 __syncwarp();
                 if (lane == 0) {
@@ -480,21 +462,16 @@ __device__ __forceinline__ void fast_swiglu_tile(const GemmDev& p, const CUtenso
         }
         fence_proxy_async_smem();
         __syncwarp();
-        if (lane == 0 && !(p.dbg & 1)) {
+        if (lane == 0) {
             tma_store_2d(tmO, stg2, (n0 >> 1) + 64 * hsel, m0 + q * 32);
             bulk_commit();
         }
-    } else {
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) arrive_tempty<G2>(tempty);
     }
 }
 
-template <int BN, int ACT, int FAST, bool G2>
+template <int BN, int ACT, int FAST>
 __device__ __forceinline__ void fast_epilogue_tile(const GemmDev& p, const CUtensorMap* tmO, uint8_t* stg, float* bias_s,
-                                                   int lane, int q, int hsel, uint32_t taddr, int m_blk, int n0,
-                                                   uint64_t* tfull, uint32_t aph, uint64_t* tempty) {
+                                                   int lane, int q, int hsel, const float* arow, int m_blk, int n0) {
     constexpr bool OF32 = FAST == 3 || FAST == 4;
     constexpr bool MASK = FAST == 5;
     constexpr bool RES = FAST == 2 || FAST == 4 || MASK;  // a second [M][N]-shaped operand read one chunk ahead
@@ -535,7 +512,6 @@ __device__ __forceinline__ void fast_epilogue_tile(const GemmDev& p, const CUten
                                               : make_uint4(0, 0, 0, 0);
         }
     };
-    bool waited = false;
     if (n0 + hsel * CW < N) {
         load_bias(n0 + hsel * CW);
         if (RES) {
@@ -555,25 +531,14 @@ __device__ __forceinline__ void fast_epilogue_tile(const GemmDev& p, const CUten
         const bool last = (j == NCH - 1) || (c + 2 >= TCH) || (col0 + 2 * CW >= N);
         const float b0 = b0n, b1 = b1n;
         if (!last) load_bias(col0 + 2 * CW);
-        if (!waited) {
-            mbar_wait(tfull, aph);
-            tc_fence_after();
-            waited = true;
-        }
         uint32_t r0[32], r1[32];
-        tmem_ld_32x32(taddr + c * CW, r0);
-        if (!OF32) tmem_ld_32x32(taddr + c * CW + 32, r1);
+        acc_ld32(arow + c * CW, r0);
+        if (!OF32) acc_ld32(arow + c * CW + 32, r1);
         bias_s[lane] = b0;
         if (!OF32) bias_s[32 + lane] = b1;
         if (lane == 0) bulk_wait_read0();  // the previous TMA store has finished reading the staging tile
         __syncwarp();
-        tmem_ld_wait();
-        if (last) {  // accumulator fully in registers: hand the TMEM buffer back to the MMA warp
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) arrive_tempty<G2>(tempty);
-        }
-        if (!(p.dbg & 4)) {
+        {
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
                 if constexpr (OF32) {
@@ -614,168 +579,95 @@ __device__ __forceinline__ void fast_epilogue_tile(const GemmDev& p, const CUten
                     *reinterpret_cast<uint4*>(stg + stgb_off(lane, i)) = w;
                 }
             }
-            if (RES && !last) load_resid(col0 + 2 * CW);  // in flight across the store and the next TMEM read
+            if (RES && !last) load_resid(col0 + 2 * CW);  // in flight across the store and the next accumulator read
             fence_proxy_async_smem();
             __syncwarp();
-            if (lane == 0 && !(p.dbg & 1)) {
+            if (lane == 0) {
                 if (p.conv_C) tma_store_4d(tmO, stg, col0, ctx * p.conv_TW, cty * p.conv_TH + q * (32 / p.conv_TW), cb);
                 else tma_store_2d(tmO, stg, col0, m0 + q * 32);
                 bulk_commit();
             }
         }
     }
-    if (!waited) {  // no chunk of this warp inside N: still consume the phase
-        mbar_wait(tfull, aph);
-        tc_fence_after();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) arrive_tempty<G2>(tempty);
-    }
 }
 
-// CL2: the CTA pair of a 2-CTA cluster works on two vertically adjacent tiles (same n-block): each CTA loads its own A
-// tile and HALF of the shared B tile, multicast to both — 25-33 % less L2->SMEM traffic, which is what caps this kernel
-// (128x128x64 tiles at 32 KB per k-block = 64 flop/B against ~12 TB/s of L2 is ~0.8 PFLOP/s).
-// G2 (implies CL2): ONE tcgen05.mma.cta_group::2 per k-step covers the pair's 256 x BN tile.  Each CTA stages its own A tile
-// and only HALF of B (the MMA reads both halves across the pair), so the shared-memory fill per flop drops by a third
-// against the multicast variant — the L2->SM feed is what caps the 128 x BN kernel at ~1.3 PFLOP/s.  The leader CTA's
-// MMA thread issues for both; full barriers (both CTAs' TMA bytes) and accumulator-empty barriers live in the leader.
-// Wider clusters (4 / 8 CTAs sharing one B tile) were built and measured in round 2 (profiles/r2_gemm_cluster_width.md):
-// slower than the pair on every shape of the step (fc1 197 -> 203 -> 216 us), so only the pair remains.
-// BRES (implicit conv, 64 input channels -> <= 64 output channels; the two 64-channel VGG layers at 256 x 256 were bound by
-// the L2->SM feed: 9 taps x (16 KB pixels + 16 KB weights) per 128-pixel tile):
-//   1: the whole [BN x 9*64] weight matrix (72 KB) is loaded ONCE per CTA and stays resident; the ring carries only A;
-//   2: additionally the A operand is loaded once per tile as a (16+2) x 16-pixel HALO block (36 KB; tile = 16 rows x 8 pixels)
-//      and the nine taps are row-shifted UMMA descriptors into it (start + dy*2048 + dx*128, SBO = 2048): 8x less feed.
-//   3: any channel count (multiple of 64) and tile width: TWO rings — a 2-stage ring of halo blocks (one per 64-channel block
-//      of the tile, used by nine taps) and a STAGES-deep ring of [BN x 64] weight k-blocks (pair multicast as before), k-order
-//      (channel block, tap).  A-operand feed per tile drops from 9 x 16 KB to 36 KB per 64 channels.
-template <int BN, int STAGES, int ACT, bool PS, bool CL2, int MINB, int FAST, bool G2, int BRES = 0>
-// 10 warps -> 3 on one scheduler: 3*32*R <= 16384 registers per SM sub-partition caps R at 168 (MINB = 1).
-// MINB = 2 (short-K shapes): two CTAs per SM with a 2-stage ring double the epilogue warps per SM at ~100 registers.
-__global__ void __launch_bounds__(NUM_THREADS, MINB)
+// Consumer mainloop of one tile: warpgroup wg multiplies rows [64 wg, 64 wg + 64) of the tile.  One wgmma group stays in
+// flight; a ring slot is released (one arrival per consumer warp) once the group that read it has completed.
+template <int BN, int STAGES, int TA, int TB>
+__device__ __forceinline__ void gemm_mainloop(float (&acc)[BN / 2], uint8_t* ring, uint64_t* full_bar, uint64_t* empty_bar,
+                                              int& s, uint32_t& ph, int nkb, int wg, int lane) {
+    constexpr int STAGE_BYTES = A_BYTES + BN * BK * 2;
+    int prev = -1;
+    for (int kb = 0; kb < nkb; ++kb) {
+        mbar_wait(&full_bar[s], ph);
+        const uint32_t a_base = smem_u32(ring + s * STAGE_BYTES) + wg * 8192;  // K- or MN-major: 64 rows of A = 8 KB
+        const uint32_t b_base = smem_u32(ring + s * STAGE_BYTES + A_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int j = 0; j < BK / 16; ++j) {
+            const uint64_t ad = TA ? wgmma_desc_sw128(a_base + j * 2048, 8192, 1024) : wgmma_desc_sw128(a_base + j * 32, 0, 1024);
+            const uint64_t bd = TB ? wgmma_desc_sw128(b_base + j * 2048, 8192, 1024) : wgmma_desc_sw128(b_base + j * 32, 0, 1024);
+            const uint32_t sc = (kb > 0 || j > 0) ? 1u : 0u;
+            if constexpr (BN == 128) wgmma_m64n128_ss<TA, TB>(acc, ad, bd, sc);
+            else wgmma_m64n64_ss<TA, TB>(acc, ad, bd, sc);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        fence_regs(acc);
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        prev = s;
+        if (++s == STAGES) s = 0, ph ^= 1;
+    }
+    wgmma_wait<0>();
+    fence_regs(acc);
+    if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+}
+
+template <int BN, int STAGES, int ACT, bool PS, int FAST>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
             const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmO2, const GemmDev p) {
-    static_assert(!G2 || CL2, "cta_group::2 needs the 2-CTA cluster");
-    constexpr int CLM = 2;                                      // CTAs per cluster (along M) sharing one B tile
-    constexpr uint16_t MC_MASK = (uint16_t)((1u << CLM) - 1u);  // every CTA of the cluster
-    constexpr bool RESB = BRES == 1 || BRES == 2;  // resident weights
-    static_assert(!RESB || (!CL2 && !G2 && FAST != 0 && BN == 64), "resident-B conv form: 64-wide lean-epilogue tiles");
-    static_assert(BRES != 3 || (!G2 && FAST != 0), "two-ring halo conv form: lean epilogue, no cta_group::2");
-    constexpr bool ALT_EPI = BRES != 0 && BN == 64;  // one column chunk per tile: the epilogue warp groups alternate tiles
-    constexpr int AST = 2;                           // BRES == 3: halo-block stages
-    constexpr int A_ST_BYTES = BRES == 2 ? HALO_BYTES : (BRES == 3 ? 0 : A_BYTES);
-    constexpr int B_BYTES = RESB ? 0 : (G2 ? BN / 2 : BN) * BK * 2;
-    constexpr int STAGE_BYTES = A_ST_BYTES + B_BYTES;
-    // in front of the ring: the resident weights (1, 2) or the halo-block ring (3)
-    constexpr int BRES_BYTES = RESB ? BRES_KB * BN * BK * 2 : (BRES == 3 ? AST * HALO_BYTES : 0);
-    constexpr int ACC_STRIDE = BN == 192 ? 256 : BN;  // column distance of the two accumulator buffers
-    constexpr uint32_t TMEM_COLS = 2 * ACC_STRIDE;    // 256 or 512 (power of two)
-
-    // FAST kernels use every byte (ring + staging + bias tiles + barriers = 226 KB at BN = 256): they rely on the declared
-    // 1024-byte alignment of the dynamic segment (checked below) instead of carrying a 1 KB alignment pad
+    static_assert(BN == 64 || BN == 128, "tile width");
+    constexpr int B_BYTES = BN * BK * 2;
+    constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+    constexpr int ACC_LD = BN + 4;  // padded fp32 accumulator rows
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* smem = FAST ? smem_raw
-                         : reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    if (FAST && (smem_u32(smem_raw) & 1023u) != 0u) __trap();
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     constexpr int STG_BYTES = NUM_EPI_WARPS * STG_FLOATS * 4 * (FAST == 6 ? 2 : 1);  // FAST 6: + the hidden-tile staging
-    uint8_t* ring = smem + BRES_BYTES;
-    float* stg_base = reinterpret_cast<float*>(ring + STAGES * STAGE_BYTES);  // 8 epilogue warps x 4 KB
-    float* bias_base = reinterpret_cast<float*>(ring + STAGES * STAGE_BYTES + STG_BYTES);  // FAST only
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(ring + STAGES * STAGE_BYTES + STG_BYTES + (FAST ? NUM_EPI_WARPS * 256 : 0));
+    uint8_t* ring = smem;
+    float* acc_s = reinterpret_cast<float*>(ring + STAGES * STAGE_BYTES);
+    float* stg_base = acc_s + BM * ACC_LD;                                                 // 8 epilogue warps x 4 KB
+    float* bias_base = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(stg_base) + STG_BYTES);  // FAST only
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(bias_base) + (FAST ? NUM_EPI_WARPS * 256 : 0));
     uint64_t* empty_bar = full_bar + STAGES;
-    uint64_t* tfull_bar = empty_bar + STAGES;
-    uint64_t* tempty_bar = tfull_bar + 2;
-    uint64_t* bres_bar = tempty_bar + 2;  // BRES 1, 2: the resident weights have landed
-    uint64_t* afull_bar = bres_bar + 1;   // BRES 3: [AST] halo block landed
-    uint64_t* aempty_bar = afull_bar + 2; // BRES 3: [AST] halo block consumed by its nine taps
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(aempty_bar + 2);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const uint32_t crank = CL2 ? cluster_ctarank() : 0u;
-    const int work_id = CL2 ? (blockIdx.x / CLM) : blockIdx.x;      // the CTAs of a cluster share a work item (CLM tiles)
-    const int work_stride = CL2 ? (gridDim.x / CLM) : gridDim.x;
+    const int work_id = blockIdx.x;
+    const int work_stride = gridDim.x;
 
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
         if (FAST) tma_prefetch_desc(&tmO);
         if (FAST == 6) tma_prefetch_desc(&tmO2);
-        for (int s = 0; s < STAGES; ++s) mbar_init(&full_bar[s], 1), mbar_init(&empty_bar[s], (CL2 && !G2) ? CLM : 1);
-        for (int s = 0; s < 2; ++s)
-            mbar_init(&tfull_bar[s], 1),
-                mbar_init(&tempty_bar[s], ALT_EPI ? NUM_EPI_WARPS / 2 : (G2 ? 2 * NUM_EPI_WARPS : NUM_EPI_WARPS));
-        mbar_init(bres_bar, 1);
-        for (int s = 0; s < 2; ++s) mbar_init(&afull_bar[s], 1), mbar_init(&aempty_bar[s], 1);
+        for (int s = 0; s < STAGES; ++s) mbar_init(&full_bar[s], 1), mbar_init(&empty_bar[s], NUM_EPI_WARPS);
         fence_barrier_init();
     }
-    if (warp == 1) {
-        if (G2) tmem_alloc_g2(tmem_slot, TMEM_COLS), tmem_relinquish_g2();
-        else tmem_alloc(tmem_slot, TMEM_COLS), tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    if (CL2) cluster_sync_all();  // peer barriers are initialised before anything is multicast into this CTA
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    // in CL2 mode num_m_blocks counts tile PAIRS; this CTA's m-block is 2*pair + rank
     const int tiles_mn = p.num_m_blocks * p.num_n_blocks;
     const int num_tiles = tiles_mn * p.num_splits;
 
-    if (warp == 0) {
+    if (warp < 4) {
         // ============================== TMA producer ==============================
-        if (lane == 0) {
+        setmaxnreg_dec<40>();
+        if (warp == 0 && lane == 0) {
             int s = 0;
             uint32_t ph = 0;
-            [[maybe_unused]] int sa_ = 0;
-            [[maybe_unused]] uint32_t aph_ = 0;
             TileIter ti(work_id, work_stride, p.num_n_blocks, p.num_m_blocks);
-            if constexpr (RESB) {  // the whole weight matrix, once (N <= BN: rows beyond N are zero-filled)
-                mbar_expect_tx(bres_bar, BRES_BYTES);
-#pragma unroll
-                for (int kb = 0; kb < BRES_KB; ++kb) tma_load_2d(smem + kb * (BN * BK * 2), &tmB, bres_bar, kb * BK, 0);
-            }
             for (int t = work_id; t < num_tiles; t += work_stride, ti.next()) {
-                const int n_blk = ti.n;
-                const int m_blk = ti.m * (CL2 ? CLM : 1) + (int)crank;
-                if constexpr (BRES == 2) {  // one halo block per tile: pixels (x0-1 .. x0+14) x (y0-1 .. y0+16), zero fill = padding
-                    const int hx0 = (m_blk % p.conv_tiles_w) * p.conv_TW;
-                    const int hy0 = ((m_blk / p.conv_tiles_w) % p.conv_tiles_h) * p.conv_TH;
-                    const int hb = m_blk / (p.conv_tiles_w * p.conv_tiles_h);
-                    mbar_wait(&empty_bar[s], ph ^ 1);
-                    mbar_expect_tx(&full_bar[s], HALO_BYTES);
-                    tma_load_4d(ring + s * STAGE_BYTES, &tmA, &full_bar[s], 0, hx0 - 1, hy0 - 1, hb);
-                    if (++s == STAGES) s = 0, ph ^= 1;
-                    continue;
-                }
-                if constexpr (BRES == 3) {  // per 64-channel block: one halo block, then its nine [BN x 64] weight k-blocks
-                    const int hx0 = (m_blk % p.conv_tiles_w) * p.conv_TW;
-                    const int hy0 = ((m_blk / p.conv_tiles_w) % p.conv_tiles_h) * p.conv_TH;
-                    const int hb = m_blk / (p.conv_tiles_w * p.conv_tiles_h);
-                    const int n0h = n_blk * BN;
-                    for (int c0 = 0; c0 < p.conv_C; c0 += 64) {
-                        mbar_wait(&aempty_bar[sa_], aph_ ^ 1);
-                        mbar_expect_tx(&afull_bar[sa_], HALO_BYTES);
-                        tma_load_4d(smem + sa_ * HALO_BYTES, &tmA, &afull_bar[sa_], c0, hx0 - 1, hy0 - 1, hb);
-                        if (++sa_ == AST) sa_ = 0, aph_ ^= 1;
-#pragma unroll 1
-                        for (int tap = 0; tap < 9; ++tap) {
-                            mbar_wait(&empty_bar[s], ph ^ 1);
-                            mbar_expect_tx(&full_bar[s], STAGE_BYTES);  // the whole k-block (in a pair: both halves land here)
-                            uint8_t* sb = ring + s * STAGE_BYTES;
-                            const int k0 = tap * p.conv_C + c0;
-                            if (CL2)
-                                tma_load_2d_mc(sb + crank * (BN / CLM) * 128, &tmB, &full_bar[s], k0, n0h + (int)crank * (BN / CLM),
-                                               MC_MASK);
-                            else tma_load_2d(sb, &tmB, &full_bar[s], k0, n0h);
-                            if (++s == STAGES) s = 0, ph ^= 1;
-                        }
-                    }
-                    continue;
-                }
-                const int ks = ti.ks;
+                const int n_blk = ti.n, m_blk = ti.m, ks = ti.ks;
                 const int kb0 = ks * p.kb_per_split;
                 const int kb1 = min(kb0 + p.kb_per_split, p.num_k_blocks);
                 const int m0 = m_blk * BM, n0 = n_blk * BN;
@@ -795,9 +687,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                     mbar_wait(&empty_bar[s], ph ^ 1);
                     uint8_t* sa = ring + s * STAGE_BYTES;
                     uint8_t* sb = sa + A_BYTES;
-                    if (!G2) mbar_expect_tx(&full_bar[s], STAGE_BYTES);
-                    else if (crank == 0) mbar_expect_tx(&full_bar[s], 2 * STAGE_BYTES);  // both CTAs' bytes land here
-                    const uint32_t lbar = G2 ? mapa_u32(&full_bar[s], 0) : 0u;
+                    mbar_expect_tx(&full_bar[s], STAGE_BYTES);
                     const int k0 = kb * BK;
                     if (p.conv_C) {
                         tma_load_4d(sa, &tmA, &full_bar[s], cv_c, cv_x0 + cv_dx, cv_y0 + cv_dy, cv_b);
@@ -806,188 +696,72 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                             cv_c = 0;
                             if (++cv_dx == 2) cv_dx = -1, ++cv_dy;
                         }
-                    } else if (G2) {
-                        if (!p.a_mn) {
-                            tma_load_2d_g2(sa, &tmA, lbar, k0, m0);
-                        } else {
-                            tma_load_2d_g2(sa, &tmA, lbar, m0, k0);
-                            tma_load_2d_g2(sa + 8192, &tmA, lbar, m0 + 64, k0);
-                        }
                     } else if (!p.a_mn) {
                         tma_load_2d(sa, &tmA, &full_bar[s], k0, m0);
                     } else {
                         tma_load_2d(sa, &tmA, &full_bar[s], m0, k0);
                         tma_load_2d(sa + 8192, &tmA, &full_bar[s], m0 + 64, k0);
                     }
-                    if constexpr (RESB) {
-                        // weights are resident
-                    } else if (G2) {  // my half of B stays in MY shared memory: the pair's MMA reads both halves
-                        if (!p.b_mn) {
-                            tma_load_2d_g2(sb, &tmB, lbar, k0, n0 + (int)crank * (BN / 2));
-                        } else {
-#pragma unroll
-                            for (int i = 0; i < BN / 128; ++i)
-                                tma_load_2d_g2(sb + i * 8192, &tmB, lbar, n0 + ((int)crank * (BN / 128) + i) * 64, k0);
-                        }
-                    } else if (CL2) {  // my 1/CLM of B, delivered to every CTA of the cluster
-                        if (!p.b_mn) {
-                            tma_load_2d_mc(sb + crank * (BN / CLM) * 128, &tmB, &full_bar[s], k0, n0 + (int)crank * (BN / CLM),
-                                           MC_MASK);
-                        } else {
-#pragma unroll
-                            for (int i = 0; i < BN / 64; ++i)   // MN-major B: whole 64-column chunks, dealt out alternately
-                                if ((i % CLM) == (int)crank)
-                                    tma_load_2d_mc(sb + i * 8192, &tmB, &full_bar[s], n0 + 64 * i, k0, MC_MASK);
-                        }
-                    } else if (!p.b_mn) {
+                    if (!p.b_mn) {
                         tma_load_2d(sb, &tmB, &full_bar[s], k0, n0);
                     } else {
 #pragma unroll
-                        for (int i = 0; i < BN / 64; ++i)
-                            tma_load_2d(sb + i * 8192, &tmB, &full_bar[s], n0 + 64 * i, k0);
+                        for (int i = 0; i < BN / 64; ++i) tma_load_2d(sb + i * 8192, &tmB, &full_bar[s], n0 + 64 * i, k0);
                     }
                     if (++s == STAGES) s = 0, ph ^= 1;
                 }
-            }
-        }
-    } else if (warp == 1) {
-        // ============================== UMMA issuer ==============================
-        if (lane == 0 && (!G2 || crank == 0)) {
-            const uint32_t idesc = umma_idesc_bf16(G2 ? 2 * BM : BM, BN, p.a_mn, p.b_mn);
-            int s = 0;
-            uint32_t ph = 0;
-            int as = 0;
-            uint32_t aph = 0;
-            TileIter ti(work_id, work_stride, p.num_n_blocks, p.num_m_blocks);
-            if constexpr (RESB) {
-                mbar_wait(bres_bar, 0);
-                tc_fence_after();
-            }
-            [[maybe_unused]] int sa_ = 0;
-            [[maybe_unused]] uint32_t aph_ = 0;
-            for (int t = work_id; t < num_tiles; t += work_stride, ti.next()) {
-                const int ks = ti.ks;
-                const int kb0 = ks * p.kb_per_split;
-                const int kb1 = min(kb0 + p.kb_per_split, p.num_k_blocks);
-                mbar_wait(&tempty_bar[as], aph ^ 1);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + as * ACC_STRIDE;
-                if constexpr (BRES == 2) {  // nine taps = nine row-shifted windows of the halo block, K = 64 each
-                    mbar_wait(&full_bar[s], ph);
-                    tc_fence_after();
-                    const uint32_t a_base = smem_u32(ring + s * STAGE_BYTES);
-                    const uint32_t w_base = smem_u32(smem);
-#pragma unroll
-                    for (int tap = 0; tap < 9; ++tap) {
-                        const int dy = tap / 3, dx = tap % 3;
-#pragma unroll
-                        for (int j = 0; j < BK / 16; ++j) {
-                            // 8-row groups = 8 consecutive pixels of one tile row (halo row pitch 16 pixels = 2048 B = SBO).  The dx
-                            // shift starts each group dx 128-byte rows into the 1024-byte swizzle pattern; the descriptor's
-                            // base-offset field stays 0: the 128B swizzle is a function of the absolute shared-memory address
-                            // bits (measured: base offset = dx gives wrong products, 0 is exact — profiles/r2_conv_halo.md)
-                            const uint64_t ad = umma_desc_sw128(a_base + dy * (HALO_W * 128) + dx * 128 + j * 32, 0, HALO_W * 128);
-                            const uint64_t bd = umma_desc_sw128(w_base + tap * (BN * BK * 2) + j * 32, 0, 1024);
-                            if (p.dbg & 8) continue;
-                            umma_bf16_ss(d_tmem, ad, bd, idesc, (tap > 0 || j > 0) ? 1u : 0u);
-                        }
-                    }
-                    umma_commit(&empty_bar[s]);
-                    if (++s == STAGES) s = 0, ph ^= 1;
-                }
-                if constexpr (BRES == 3) {
-                    for (int c0 = 0; c0 < p.conv_C; c0 += 64) {
-                        mbar_wait(&afull_bar[sa_], aph_);
-                        tc_fence_after();
-                        const uint32_t a_base = smem_u32(smem + sa_ * HALO_BYTES);
-#pragma unroll
-                        for (int tap = 0; tap < 9; ++tap) {
-                            const int dy = tap / 3, dx = tap % 3;
-                            mbar_wait(&full_bar[s], ph);
-                            tc_fence_after();
-                            const uint32_t b_base = smem_u32(ring + s * STAGE_BYTES);
-#pragma unroll
-                            for (int j = 0; j < BK / 16; ++j) {
-                                const uint64_t ad = umma_desc_sw128(a_base + dy * (HALO_W * 128) + dx * 128 + j * 32, 0, HALO_W * 128);
-                                const uint64_t bd = umma_desc_sw128(b_base + j * 32, 0, 1024);
-                                if (p.dbg & 8) continue;
-                                umma_bf16_ss(d_tmem, ad, bd, idesc, (c0 > 0 || tap > 0 || j > 0) ? 1u : 0u);
-                            }
-                            if (CL2) umma_commit_mc(&empty_bar[s], MC_MASK);   // the peer multicasts into my slot too
-                            else umma_commit(&empty_bar[s]);
-                            if (++s == STAGES) s = 0, ph ^= 1;
-                        }
-                        umma_commit(&aempty_bar[sa_]);  // local: the halo ring is not shared
-                        if (++sa_ == AST) sa_ = 0, aph_ ^= 1;
-                    }
-                }
-                for (int kb = kb0; BRES < 2 && kb < kb1; ++kb) {
-                    mbar_wait(&full_bar[s], ph);
-                    tc_fence_after();
-                    const uint32_t a_base = smem_u32(ring + s * STAGE_BYTES);
-                    const uint32_t b_base = RESB ? smem_u32(smem) + kb * (BN * BK * 2) : a_base + A_BYTES;
-#pragma unroll
-                    for (int j = 0; j < BK / 16; ++j) {
-                        const uint64_t ad = p.a_mn ? umma_desc_sw128(a_base + j * 2048, 8192, 1024)
-                                                   : umma_desc_sw128(a_base + j * 32, 0, 1024);
-                        const uint64_t bd = p.b_mn ? umma_desc_sw128(b_base + j * 2048, 8192, 1024)
-                                                   : umma_desc_sw128(b_base + j * 32, 0, 1024);
-                        if (p.dbg & 8) continue;
-                        if (G2) umma_bf16_ss_g2(d_tmem, ad, bd, idesc, (kb > kb0 || j > 0) ? 1u : 0u);
-                        else umma_bf16_ss(d_tmem, ad, bd, idesc, (kb > kb0 || j > 0) ? 1u : 0u);
-                    }
-                    // frees the smem slot once these MMAs have read it (in both CTAs: the peer multicasts into mine)
-                    if (G2) umma_commit_mc_g2(&empty_bar[s], 3);
-                    else if (CL2) umma_commit_mc(&empty_bar[s], MC_MASK);
-                    else umma_commit(&empty_bar[s]);
-                    if (++s == STAGES) s = 0, ph ^= 1;
-                }
-                // accumulator complete (with cta_group::2: in both CTAs, each runs its own epilogue on its 128 rows)
-                if (G2) umma_commit_mc_g2(&tfull_bar[as], 3);
-                else umma_commit(&tfull_bar[as]);
-                if (++as == 2) as = 0, aph ^= 1;
             }
         }
     } else {
-        // ============================== epilogue (warps 2..9) ==============================
-        const int q = warp & 3;            // TMEM lane quarter this warp may access
-        const int hsel = (warp - 2) >> 2;  // parity of the 64-column units this warp handles
-        float* stg = stg_base + (warp - 2) * STG_FLOATS;
+        // ============================== consumers: wgmma mainloop, then the epilogue ==============================
+        setmaxnreg_inc<232>();
+        const int wg = (warp >> 2) - 1;    // consumer warpgroup: tile rows [64 wg, 64 wg + 64)
+        const int q = warp & 3;            // row quarter of the tile this warp runs the epilogue for
+        const int hsel = (warp - 4) >> 2;  // parity of the 64-column units this warp handles
+        const int tw = threadIdx.x & 127;
+        float* stg = stg_base + (warp - 4) * STG_FLOATS;
         const bool has_resid = p.resid != nullptr;
-        int as = 0;
-        uint32_t aph = 0;
+        const float* arow = acc_s + (q * 32 + lane) * ACC_LD;
+        int s = 0;
+        uint32_t ph = 0;
         TileIter ti(work_id, work_stride, p.num_n_blocks, p.num_m_blocks);
         for (int t = work_id; t < num_tiles; t += work_stride, ti.next()) {
-            const int n_blk = ti.n;
-            const int m_blk = ti.m * (CL2 ? CLM : 1) + (int)crank;
+            const int n_blk = ti.n, m_blk = ti.m, ks = ti.ks;
+            const int kb0 = ks * p.kb_per_split;
+            const int nkb = min(kb0 + p.kb_per_split, p.num_k_blocks) - kb0;
+            float acc[BN / 2];
+            if (p.a_mn) {
+                if (p.b_mn) gemm_mainloop<BN, STAGES, 1, 1>(acc, ring, full_bar, empty_bar, s, ph, nkb, wg, lane);
+                else gemm_mainloop<BN, STAGES, 1, 0>(acc, ring, full_bar, empty_bar, s, ph, nkb, wg, lane);
+            } else {
+                if (p.b_mn) gemm_mainloop<BN, STAGES, 0, 1>(acc, ring, full_bar, empty_bar, s, ph, nkb, wg, lane);
+                else gemm_mainloop<BN, STAGES, 0, 0>(acc, ring, full_bar, empty_bar, s, ph, nkb, wg, lane);
+            }
+            // accumulators -> padded fp32 tile (the previous tile's epilogue has finished reading it)
+            asm volatile("bar.sync 1, 256;" ::: "memory");
+            {
+                const int r0 = 64 * wg + 16 * (tw >> 5) + ((tw & 31) >> 2), c0 = 2 * (tw & 3);
+#pragma unroll
+                for (int j = 0; j < BN / 8; ++j) {
+                    *reinterpret_cast<float2*>(acc_s + r0 * ACC_LD + 8 * j + c0) = make_float2(acc[4 * j], acc[4 * j + 1]);
+                    *reinterpret_cast<float2*>(acc_s + (r0 + 8) * ACC_LD + 8 * j + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+                }
+            }
+            asm volatile("bar.sync 1, 256;" ::: "memory");
             const int m0 = m_blk * BM, n0 = n_blk * BN;
             const int grow0 = m0 + q * 32;
-            const uint32_t taddr = tmem_base + (uint32_t(q * 32) << 16) + as * ACC_STRIDE;
             if constexpr (FAST == 6 || FAST == 7) {
                 uint8_t* st1 = reinterpret_cast<uint8_t*>(stg);
                 // FAST 6: second tile behind the eight pre-activation tiles; FAST 7: the only tile holds the hidden values
-                uint8_t* st2 = FAST == 6 ? reinterpret_cast<uint8_t*>(stg_base) + (NUM_EPI_WARPS + (warp - 2)) * STG_FLOATS * 4 : st1;
-                fast_swiglu_tile<BN, FAST, G2>(p, &tmO, &tmO2, st1, st2, bias_base + (warp - 2) * 64, lane, q, hsel, taddr, m_blk,
-                                               n0, &tfull_bar[as], aph, &tempty_bar[as]);
-                if (++as == 2) as = 0, aph ^= 1;
-                continue;
-            }
-            if constexpr (ALT_EPI) {
-                // 64-wide tiles are one column chunk: instead of idling every second warp, the two warps of a lane quarter
-                // take alternate tiles (warp group hsel owns accumulator buffer hsel; 4 arrivals free a buffer)
-                if (hsel == as)
-                    fast_epilogue_tile<BN, ACT, FAST, G2>(p, &tmO, reinterpret_cast<uint8_t*>(stg), bias_base + (warp - 2) * 64,
-                                                          lane, q, 0, taddr, m_blk, n0, &tfull_bar[as], aph, &tempty_bar[as]);
-                if (++as == 2) as = 0, aph ^= 1;
+                uint8_t* st2 = FAST == 6 ? reinterpret_cast<uint8_t*>(stg_base) + (NUM_EPI_WARPS + (warp - 4)) * STG_FLOATS * 4 : st1;
+                fast_swiglu_tile<BN, FAST>(p, &tmO, &tmO2, st1, st2, bias_base + (warp - 4) * 64, lane, q, hsel, arow, m_blk, n0);
                 continue;
             }
             if constexpr (FAST != 0) {
-                fast_epilogue_tile<BN, ACT, FAST, G2>(p, &tmO, reinterpret_cast<uint8_t*>(stg), bias_base + (warp - 2) * 64, lane,
-                                                  q, hsel, taddr, m_blk, n0, &tfull_bar[as], aph, &tempty_bar[as]);
-                if (++as == 2) as = 0, aph ^= 1;
+                fast_epilogue_tile<BN, ACT, FAST>(p, &tmO, reinterpret_cast<uint8_t*>(stg), bias_base + (warp - 4) * 64, lane, q,
+                                                  hsel, arow, m_blk, n0);
                 continue;
             }
-            bool waited = false;
             constexpr bool sw = ACT == VTP_ACT_SWIGLU8;
             long orow8[8];  // output rows of the cooperative store pattern (row 4*it + lane/8 of this warp's slab)
 #pragma unroll
@@ -997,90 +771,43 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             uint32_t hold[16];  // first half of a SwiGLU hidden line, kept in registers until its partner unit is done
 #pragma unroll 1
             for (int j = 0; j < BN / 64; ++j) {
-                const int u = sw ? (BN >= 256 ? 2 * hsel + j : (hsel == 0 ? j : BN / 64)) : hsel + 2 * j;
+                const int u = sw ? (hsel == 0 ? j : BN / 64) : hsel + 2 * j;
                 if (u >= BN / 64) break;
                 const int col0 = n0 + u * 64;
                 if (col0 >= p.N) break;  // warp-uniform
-                if (has_resid)  // pull the residual lines into L2 while the accumulator is still being produced
+                if (has_resid)  // pull the residual lines into L2 before they are read
                     prefetch_resid_l2(p, lane, orow8, sw ? col0 >> 1 : col0, sw ? 32 : 64, sw ? p.N >> 1 : p.N);
-                if (!waited) {
-                    mbar_wait(&tfull_bar[as], aph);
-                    tc_fence_after();
-                    waited = true;
-                }
-                if (p.dbg & 4) continue;
                 uint32_t r0[32], r1[32];
-                if (!(p.dbg & 2)) {
-                    tmem_ld_32x32(taddr + u * 64, r0);
-                    tmem_ld_32x32(taddr + u * 64 + 32, r1);
-                    tmem_ld_wait();
-                } else {
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) r0[i] = r1[i] = 0;
-                }
+                acc_ld32(arow + u * 64, r0);
+                acc_ld32(arow + u * 64 + 32, r1);
                 float v[64];
 #pragma unroll
                 for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r0[i]), v[32 + i] = __uint_as_float(r1[i]);
                 epilogue_unit<ACT, PS>(p, stg, lane, v, grow0, orow8, col0, has_resid, sw ? (u & 1) : 0, hold);
             }
-            if (!waited) {  // this warp had no unit in the tile (N tail): still consume the phase
-                mbar_wait(&tfull_bar[as], aph);
-                tc_fence_after();
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) arrive_tempty<G2>(&tempty_bar[as]);
-            if (++as == 2) as = 0, aph ^= 1;
         }
-    }
-
-    if (FAST && warp >= 2 && lane == 0) bulk_wait0();  // outstanding TMA stores of this warp
-    tc_fence_before();
-    __syncthreads();
-    if (CL2) cluster_sync_all();  // no CTA may exit while its peer can still multicast into it / arrive on its barriers
-    if (warp == 1) {
-        tc_fence_after();
-        if (G2) tmem_dealloc_g2(tmem_base, TMEM_COLS);
-        else tmem_dealloc(tmem_base, TMEM_COLS);
+        if (FAST && lane == 0) bulk_wait0();  // outstanding TMA stores of this warp
     }
 }
 
-template <int BN, int STAGES, int ACT, bool PS, bool CL2, int MINB, int FAST = 0, bool G2 = false, int BRES = 0>
+template <int BN, int STAGES, int ACT, bool PS, int FAST = 0>
 static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& p, cudaStream_t stream,
                        const CUtensorMap* tmO = nullptr, const CUtensorMap* tmO2 = nullptr) {
-    constexpr int stage_bytes = BRES == 2 ? HALO_BYTES
-                                : (BRES == 1 ? A_BYTES : (BRES == 3 ? BN * BK * 2 : A_BYTES + (G2 ? BN / 2 : BN) * BK * 2));
-    constexpr int front_bytes = (BRES == 1 || BRES == 2) ? BRES_KB * BN * BK * 2 : (BRES == 3 ? 2 * HALO_BYTES : 0);
-    constexpr int smem_bytes = front_bytes + STAGES * stage_bytes +
-                               NUM_EPI_WARPS * STG_FLOATS * 4 * (FAST == 6 ? 2 : 1) + (FAST ? NUM_EPI_WARPS * 256 + 256 : 1024 + 256);
-    static_assert(smem_bytes <= 232448, "shared memory budget");
+    constexpr int smem_bytes = 1024 + STAGES * (A_BYTES + BN * BK * 2) + BM * (BN + 4) * 4 +
+                               NUM_EPI_WARPS * STG_FLOATS * 4 * (FAST == 6 ? 2 : 1) + (FAST ? NUM_EPI_WARPS * 256 : 0) +
+                               2 * STAGES * 8;
+    static_assert(smem_bytes <= 232448, "shared memory budget (227 KB per block)");
     static bool configured = false;
     if (!configured) {
-        VTP_CUDA(cudaFuncSetAttribute(gemm_kernel<BN, STAGES, ACT, PS, CL2, MINB, FAST, G2, BRES>,
-                                      cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+        VTP_CUDA(cudaFuncSetAttribute(gemm_kernel<BN, STAGES, ACT, PS, FAST>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      smem_bytes));
         configured = true;
     }
-    const int work = p.num_m_blocks * p.num_n_blocks * p.num_splits;  // tiles, or tile pairs in CL2 mode
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cudaLaunchAttribute attr[1];
-    constexpr int CLM = 2;
-    if (CL2) {
-        const int groups = MINB * num_sms() / CLM;  // co-resident clusters of the persistent grid
-        cfg.blockDim = dim3(NUM_THREADS);
-        cfg.dynamicSmemBytes = smem_bytes;
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = CLM, attr[0].val.clusterDim.y = 1, attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr, cfg.numAttrs = 1;
-        cfg.gridDim = dim3(CLM * (work < groups ? work : groups));
-    } else {
-        cfg.gridDim = dim3(work < MINB * num_sms() ? work : MINB * num_sms());
-    }
-    cfg.blockDim = dim3(NUM_THREADS);
-    cfg.dynamicSmemBytes = smem_bytes;
-    cfg.stream = stream;
-    VTP_CUDA(cudaLaunchKernelEx(&cfg, gemm_kernel<BN, STAGES, ACT, PS, CL2, MINB, FAST, G2, BRES>, tmA, tmB, tmO ? *tmO : tmA,
-                                tmO2 ? *tmO2 : tmA, p));
+    const int work = p.num_m_blocks * p.num_n_blocks * p.num_splits;
+    const int grid = work < num_sms() ? work : num_sms();  // persistent: one CTA per SM
+    gemm_kernel<BN, STAGES, ACT, PS, FAST><<<grid, NUM_THREADS, smem_bytes, stream>>>(tmA, tmB, tmO ? *tmO : tmA,
+                                                                                     tmO2 ? *tmO2 : tmA, p);
+    VTP_LAUNCH_CHECK();
     return VTP_OK;
 }
 
@@ -1121,16 +848,8 @@ extern "C" int vtp_gemm_bf16(const vtp_gemm_args* a, vtp_stream_t stream_) {
                       "gemm(conv): need C %% 64 == 0, W %% 4 == 0, K == 9*C, M == B*H*W");
     }
     if (a->mask_pos) VTP_CHECK_ARG(a->out_dtype == VTP_BF16 && a->ldm % 8 == 0, "gemm: mask_pos needs bf16 out");
-    // tile-N choice: minimise padded N, ties -> 256 (lower smem bandwidth per MMA)
-    const int pad128 = ceil_div(a->N, 128) * 128, pad256 = ceil_div(a->N, 256) * 256;
-    int BN = (pad256 * 8 <= pad128 * 9) ? 256 : 128;  // accept <= 12.5 % padding for the higher-intensity tile
-    // 2-CTA multicast variant whenever there are at least two m-blocks (odd counts are padded with an all-OOB tile)
-    const bool allow_cl2 = getenv("VTP_GEMM_NO_CLUSTER") == nullptr;
-    bool cl2 = allow_cl2 && ceil_div(a->M, BM) >= 2 && !(conv && getenv("VTP_GEMM_CONV_NO_CLUSTER"));
-    // cta_group::2 (256 x BN pair tiles) wherever the 2-CTA cluster applies
-    // measured (tools/gemm_diag.py): within 3 % of the TMA-multicast variant, slightly behind on every shape (both are
-    // bound by L2->SM reads, which the two variants issue identically), so it is opt-in
-    const bool g2 = cl2 && getenv("VTP_GEMM_G2") != nullptr;
+    // 64-wide tiles when N fits in one (VGG conv1_x, 64-column projections), 128-wide otherwise
+    int BN = a->N <= 64 ? 64 : 128;
     // lean TMA-store epilogue for the recurring shapes (see fast_epilogue_tile)
     const bool allow_fast = getenv("VTP_GEMM_NO_FAST") == nullptr;
     const bool fast_conv = conv && a->out_dtype == VTP_BF16 && !a->resid && getenv("VTP_GEMM_CONV_NO_FAST") == nullptr;
@@ -1138,15 +857,16 @@ extern "C" int vtp_gemm_bf16(const vtp_gemm_args* a, vtp_stream_t stream_) {
                       (!a->mask_pos || fast_conv) && !a->accumulate && split_k == 1 &&
                       (a->act == VTP_ACT_NONE || (a->act == VTP_ACT_RELU && !a->mask_pos)) &&
                       (!a->resid || a->resid_dtype == a->out_dtype);
-    const bool plain_acc = !fast && !g2 && !conv && a->accumulate && a->act == VTP_ACT_NONE && a->ps_r == 0 &&
-                           a->rr_group == 0 && !a->out2 && !a->mask_pos && !a->resid;  // wgrad: split-K + fp32 red.add
-    if ((fast || plain_acc) && !g2 && !a->mask_pos && BN == 128 && a->N % 192 == 0 && getenv("VTP_GEMM_NO_BN192") == nullptr)
-        BN = 192;
+    // SwiGLU gate in the lean epilogue (fast_swiglu_tile): bf16 hidden output [M, N/2] (+ optional bf16 pre-activation [M, N])
+    const bool fast_swiglu = allow_fast && getenv("VTP_GEMM_NO_FAST_SWIGLU") == nullptr && a->act == VTP_ACT_SWIGLU8 && !conv &&
+                             a->out_dtype == VTP_BF16 && a->round_bf16 && !a->resid && !a->mask_pos && !a->accumulate &&
+                             split_k == 1 && a->rr_group == 0 && a->ps_r == 0 && a->ldo % 8 == 0;
+    if (a->act == VTP_ACT_SWIGLU8) BN = 128;  // a warp's packed unit pair fills one 64-column hidden line
     if (auto_split) {
-        // fill the persistent grid (148 CTAs, or 74 CTA pairs) as evenly as possible: the split with the best wave
-        // efficiency among those that keep >= 8 k-blocks per work item
-        const int grid = cl2 ? num_sms() / 2 : num_sms();
-        const int tiles = (cl2 ? ceil_div(ceil_div(a->M, BM), 2) : ceil_div(a->M, BM)) * ceil_div(a->N, BN);
+        // fill the persistent grid (one CTA per SM) as evenly as possible: the split with the best wave efficiency among
+        // those that keep >= 8 k-blocks per work item
+        const int grid = num_sms();
+        const int tiles = ceil_div(a->M, BM) * ceil_div(a->N, BN);
         const int nkb = ceil_div(a->K, BK);
         double best = -1.0;
         for (int sp = 1; sp <= 64 && sp * 8 <= (nkb > 8 ? nkb : 8); ++sp) {
@@ -1158,32 +878,6 @@ extern "C" int vtp_gemm_bf16(const vtp_gemm_args* a, vtp_stream_t stream_) {
             if (eff > best + 0.02) best = eff, split_k = sp;
         }
     }
-    // 64 -> 64-channel convs (VGG conv1_2 forward and its dgrad): resident weights (1) + halo-block A operand (2), see gemm_kernel
-    int bres = 0;
-    if (conv && fast && a->conv_C == 64 && a->N == 64 && !a->b_mn_major && !g2) {
-        bres = getenv("VTP_GEMM_CONV_BRES") ? atoi(getenv("VTP_GEMM_CONV_BRES")) : VTP_CONV_BRES_DEFAULT;
-        if (bres < 0 || bres > 2) bres = 0;
-        if (bres == 2 && a->conv_W % 8 != 0) bres = 1;
-        if (bres) BN = 64, cl2 = false;
-    }
-    // plain GEMMs with 64 output columns and K <= 576 (VGG conv1_1 through its 27 -> 32 im2col: 2.1 M rows x 64 per launch, one
-    // k-block per tile) are latency-bound per tile in the 128-wide kernel: same resident-weight 64-wide kernel, whose two
-    // epilogue warp groups take alternate tiles
-    if (!conv && fast && a->N == 64 && a->K <= BRES_KB * BK && !a->a_mn_major && !a->b_mn_major && !g2 &&
-        a->out_dtype == VTP_BF16 && !a->resid && !a->mask_pos && ceil_div(a->M, BM) >= 2 * num_sms() &&
-        getenv("VTP_GEMM_NO_N64_BRES") == nullptr)
-        bres = 1, BN = 64, cl2 = false;
-    // every other conv shape with tiles <= 128 wide: two-ring halo form (3), pair multicast of the weights kept
-    bool halo3 = false;
-    if (conv && fast && !bres && !g2 && cl2 && a->conv_W % 8 == 0 && !a->b_mn_major && BN == 128) {
-        halo3 = (getenv("VTP_GEMM_CONV_HALO") ? atoi(getenv("VTP_GEMM_CONV_HALO")) : VTP_CONV_HALO_DEFAULT) != 0;
-        if (halo3 && a->N <= 64) BN = 64;
-    }
-    const int two_max_kb = getenv("VTP_GEMM_2PERSM_MAXKB") ? atoi(getenv("VTP_GEMM_2PERSM_MAXKB")) : 16;
-    const bool short_bn128 = getenv("VTP_GEMM_SHORTK_BN128") != nullptr;
-    if (short_bn128 && ceil_div(a->K, BK) <= two_max_kb && split_k == 1 && a->conv_C == 0) BN = 128;
-
-    const int clm = 2;  // CTAs per cluster sharing one B tile (see gemm_kernel)
 
     GemmDev p;
     memset(&p, 0, sizeof(p));
@@ -1205,14 +899,12 @@ extern "C" int vtp_gemm_bf16(const vtp_gemm_args* a, vtp_stream_t stream_) {
     p.ps_r = a->ps_r, p.ps_gh = a->ps_gh, p.ps_gw = a->ps_gw, p.ps_cout = a->ps_cout;
     p.out2 = reinterpret_cast<__nv_bfloat16*>(a->out2), p.ldo2 = a->ldo2;
     p.mask_pos = reinterpret_cast<const __nv_bfloat16*>(a->mask_pos), p.ldm = a->ldm;
-    p.dbg = getenv("VTP_GEMM_DBG") ? atoi(getenv("VTP_GEMM_DBG")) : 0;
-
 
     CUtensorMap tmA, tmB;
     if (conv) {
         const int W = a->conv_W, H = a->conv_H, Cc = a->conv_C, Bimg = a->M / (H * W);
         p.conv_C = Cc, p.conv_H = H, p.conv_W = W, p.conv_B = Bimg;
-        p.conv_TW = (bres == 2 || halo3) ? 8 : ((W % 16 == 0) ? 16 : (W % 8 == 0 ? 8 : 4));
+        p.conv_TW = (W % 16 == 0) ? 16 : (W % 8 == 0 ? 8 : 4);
         p.conv_TH = 128 / p.conv_TW;
         p.conv_tiles_w = W / p.conv_TW, p.conv_tiles_h = ceil_div(H, p.conv_TH);
         p.num_m_blocks = Bimg * p.conv_tiles_h * p.conv_tiles_w;
@@ -1220,7 +912,6 @@ extern "C" int vtp_gemm_bf16(const vtp_gemm_args* a, vtp_stream_t stream_) {
         uint64_t dims[4] = {(uint64_t)Cc, (uint64_t)W, (uint64_t)H, (uint64_t)Bimg};
         uint64_t strides[3] = {(uint64_t)Cc * 2, (uint64_t)W * Cc * 2, (uint64_t)H * W * Cc * 2};
         uint32_t box[4] = {64, (uint32_t)p.conv_TW, (uint32_t)p.conv_TH, 1};
-        if (bres == 2 || halo3) box[1] = HALO_W, box[2] = HALO_H;  // the tile's pixels plus a one-pixel border (16 wide: 2048-byte rows)
         int rc = make_tmap_bf16(&tmA, a->A, 4, dims, strides, box);
         if (rc) return rc;
     } else {
@@ -1234,21 +925,12 @@ extern "C" int vtp_gemm_bf16(const vtp_gemm_args* a, vtp_stream_t stream_) {
     {
         uint64_t dims[2], strides[1] = {(uint64_t)a->ldb * 2};
         uint32_t box[2];
-        if (!p.b_mn) dims[0] = a->K, dims[1] = a->N, box[0] = 64, box[1] = (uint32_t)(cl2 ? BN / clm : BN);
+        if (!p.b_mn) dims[0] = a->K, dims[1] = a->N, box[0] = 64, box[1] = (uint32_t)BN;
         else dims[0] = a->N, dims[1] = a->K, box[0] = 64, box[1] = 64;
         int rc = make_tmap_bf16(&tmB, a->B, 2, dims, strides, box);
         if (rc) return rc;
     }
-    if (cl2) p.num_m_blocks = ceil_div(p.num_m_blocks, clm);  // groups of clm vertically adjacent tiles (pairs by default)
     // one instantiation per epilogue family keeps each kernel's code (and register pressure) small
-    // short reductions (<= 16 k-blocks) with 128-wide tiles are epilogue/latency bound: run two CTAs per SM
-    // (measured: proj+resid 237 -> 178 us, fc2+resid 244 -> 198 us at M = 131 584)
-    const bool allow_2cta = getenv("VTP_GEMM_NO_2PERSM") == nullptr;
-    const bool two = allow_2cta && BN == 128 && p.num_k_blocks <= two_max_kb && p.num_splits == 1;
-    // SwiGLU gate in the lean epilogue (fast_swiglu_tile): bf16 hidden output [M, N/2] (+ optional bf16 pre-activation [M, N])
-    const bool fast_swiglu = allow_fast && getenv("VTP_GEMM_NO_FAST_SWIGLU") == nullptr && a->act == VTP_ACT_SWIGLU8 && !conv &&
-                             !g2 && a->out_dtype == VTP_BF16 && a->round_bf16 && !a->resid && !a->mask_pos && !a->accumulate &&
-                             split_k == 1 && a->rr_group == 0 && a->ps_r == 0 && (BN == 256 || BN == 128) && a->ldo % 8 == 0;
     if (fast_swiglu) {
         CUtensorMap tmH, tmP;
         {
@@ -1262,17 +944,9 @@ extern "C" int vtp_gemm_bf16(const vtp_gemm_args* a, vtp_stream_t stream_) {
             uint32_t box[2] = {64, 32};
             int rc = make_tmap(&tmP, a->out2, VTP_BF16, 2, dims, strides, box);
             if (rc) return rc;
-            if (cl2)
-                return (BN == 256) ? launch_gemm<256, 3, VTP_ACT_SWIGLU8, false, true, 1, 6>(tmA, tmB, p, stream, &tmH, &tmP)
-                                   : launch_gemm<128, 4, VTP_ACT_SWIGLU8, false, true, 1, 6>(tmA, tmB, p, stream, &tmH, &tmP);
-            return (BN == 256) ? launch_gemm<256, 3, VTP_ACT_SWIGLU8, false, false, 1, 6>(tmA, tmB, p, stream, &tmH, &tmP)
-                               : launch_gemm<128, 4, VTP_ACT_SWIGLU8, false, false, 1, 6>(tmA, tmB, p, stream, &tmH, &tmP);
+            return launch_gemm<128, 2, VTP_ACT_SWIGLU8, false, 6>(tmA, tmB, p, stream, &tmH, &tmP);
         }
-        if (cl2)
-            return (BN == 256) ? launch_gemm<256, 4, VTP_ACT_SWIGLU8, false, true, 1, 7>(tmA, tmB, p, stream, &tmH)
-                               : launch_gemm<128, 6, VTP_ACT_SWIGLU8, false, true, 1, 7>(tmA, tmB, p, stream, &tmH);
-        return (BN == 256) ? launch_gemm<256, 4, VTP_ACT_SWIGLU8, false, false, 1, 7>(tmA, tmB, p, stream, &tmH)
-                           : launch_gemm<128, 6, VTP_ACT_SWIGLU8, false, false, 1, 7>(tmA, tmB, p, stream, &tmH);
+        return launch_gemm<128, 3, VTP_ACT_SWIGLU8, false, 7>(tmA, tmB, p, stream, &tmH);
     }
     if (fast) {
         CUtensorMap tmO;
@@ -1290,46 +964,10 @@ extern "C" int vtp_gemm_bf16(const vtp_gemm_args* a, vtp_stream_t stream_) {
         }
         if (rc) return rc;
         const int mode = a->mask_pos ? 5 : (a->out_dtype == VTP_F32 ? 3 : 1) + (a->resid ? 1 : 0);
-        if (bres) {  // conv, 64 -> 64 channels (mode 1 or 5 by construction of `fast`)
-#define VTP_BRES_CFG(ACT_, MODE_)                                                                                       \
-    return bres == 2 ? launch_gemm<64, 3, ACT_, false, false, 1, MODE_, false, 2>(tmA, tmB, p, stream, &tmO)            \
-                     : launch_gemm<64, 7, ACT_, false, false, 1, MODE_, false, 1>(tmA, tmB, p, stream, &tmO)
-            if (mode == 5) VTP_BRES_CFG(VTP_ACT_NONE, 5);
-            if (a->act == VTP_ACT_RELU) VTP_BRES_CFG(VTP_ACT_RELU, 1);
-            VTP_BRES_CFG(VTP_ACT_NONE, 1);
-#undef VTP_BRES_CFG
-        }
-        if (halo3) {
-#define VTP_HALO_CFG(ACT_, MODE_)                                                                                       \
-    return BN == 64 ? launch_gemm<64, 8, ACT_, false, true, 1, MODE_, false, 3>(tmA, tmB, p, stream, &tmO)              \
-                    : launch_gemm<128, 6, ACT_, false, true, 1, MODE_, false, 3>(tmA, tmB, p, stream, &tmO)
-            if (mode == 5) VTP_HALO_CFG(VTP_ACT_NONE, 5);
-            if (a->act == VTP_ACT_RELU) VTP_HALO_CFG(VTP_ACT_RELU, 1);
-            VTP_HALO_CFG(VTP_ACT_NONE, 1);
-#undef VTP_HALO_CFG
-        }
-        if (mode == 5) {  // LPIPS dgrad with the ReLU mask: bf16 out, no bias / activation
-            if (cl2)
-                return (BN == 256) ? launch_gemm<256, 4, VTP_ACT_NONE, false, true, 1, 5>(tmA, tmB, p, stream, &tmO)
-                                   : launch_gemm<128, 6, VTP_ACT_NONE, false, true, 1, 5>(tmA, tmB, p, stream, &tmO);
-            return (BN == 256) ? launch_gemm<256, 4, VTP_ACT_NONE, false, false, 1, 5>(tmA, tmB, p, stream, &tmO)
-                               : launch_gemm<128, 6, VTP_ACT_NONE, false, false, 1, 5>(tmA, tmB, p, stream, &tmO);
-        }
 #define VTP_FAST_CFG(ACT_, MODE_)                                                                                     \
-    do { /* one CTA per SM with the deep ring: measured faster than 2 x (2-stage) once the epilogue is lean */        \
-        if (g2)                                                                                                       \
-            return (BN == 256) ? launch_gemm<256, 6, ACT_, false, true, 1, MODE_, true>(tmA, tmB, p, stream, &tmO)    \
-                               : launch_gemm<128, 8, ACT_, false, true, 1, MODE_, true>(tmA, tmB, p, stream, &tmO);   \
-        if (BN == 192) {                                                                                              \
-            if (cl2) return launch_gemm<192, 4, ACT_, false, true, 1, MODE_>(tmA, tmB, p, stream, &tmO);              \
-            return launch_gemm<192, 4, ACT_, false, false, 1, MODE_>(tmA, tmB, p, stream, &tmO);                      \
-        }                                                                                                             \
-        if (cl2)                                                                                                      \
-            return (BN == 256) ? launch_gemm<256, 4, ACT_, false, true, 1, MODE_>(tmA, tmB, p, stream, &tmO)          \
-                               : launch_gemm<128, 6, ACT_, false, true, 1, MODE_>(tmA, tmB, p, stream, &tmO);         \
-        return (BN == 256) ? launch_gemm<256, 4, ACT_, false, false, 1, MODE_>(tmA, tmB, p, stream, &tmO)             \
-                           : launch_gemm<128, 6, ACT_, false, false, 1, MODE_>(tmA, tmB, p, stream, &tmO);            \
-    } while (0)
+    return BN == 64 ? launch_gemm<64, 4, ACT_, false, MODE_>(tmA, tmB, p, stream, &tmO)                              \
+                    : launch_gemm<128, 3, ACT_, false, MODE_>(tmA, tmB, p, stream, &tmO)
+        if (mode == 5) VTP_FAST_CFG(VTP_ACT_NONE, 5);  // LPIPS dgrad with the ReLU mask: bf16 out, no bias / activation
 #define VTP_FAST_ACT(ACT_)                                 \
     do {                                                   \
         switch (mode) {                                    \
@@ -1344,33 +982,17 @@ extern "C" int vtp_gemm_bf16(const vtp_gemm_args* a, vtp_stream_t stream_) {
 #undef VTP_FAST_ACT
 #undef VTP_FAST_CFG
     }
-#define VTP_LAUNCH(ACT_, PS_)                                                                                          \
-    do {                                                                                                              \
-        if (two) {                                                                                                    \
-            if (cl2) return launch_gemm<128, 2, ACT_, PS_, true, 2>(tmA, tmB, p, stream);                             \
-            return launch_gemm<128, 2, ACT_, PS_, false, 2>(tmA, tmB, p, stream);                                     \
-        }                                                                                                             \
-        if (cl2)                                                                                                      \
-            return (BN == 256) ? launch_gemm<256, 4, ACT_, PS_, true, 1>(tmA, tmB, p, stream)                         \
-                               : launch_gemm<128, 6, ACT_, PS_, true, 1>(tmA, tmB, p, stream);                        \
-        return (BN == 256) ? launch_gemm<256, 4, ACT_, PS_, false, 1>(tmA, tmB, p, stream)                            \
-                           : launch_gemm<128, 6, ACT_, PS_, false, 1>(tmA, tmB, p, stream);                           \
-    } while (0)
+#define VTP_LAUNCH(ACT_, PS_)                                                              \
+    return BN == 64 ? launch_gemm<64, 4, ACT_, PS_>(tmA, tmB, p, stream)                  \
+                    : launch_gemm<128, 3, ACT_, PS_>(tmA, tmB, p, stream)
     if (a->ps_r > 0) {
         VTP_CHECK_ARG(a->act == VTP_ACT_NONE, "gemm: pixel shuffle has no activation");
         VTP_LAUNCH(VTP_ACT_NONE, true);
     }
-    if (g2 && a->act == VTP_ACT_NONE && !(two && getenv("VTP_GEMM_G2_NOT_SHORT")))  // wgrad (split-K), logits, ...
-        return (BN == 256) ? launch_gemm<256, 6, VTP_ACT_NONE, false, true, 1, 0, true>(tmA, tmB, p, stream)
-                           : launch_gemm<128, 8, VTP_ACT_NONE, false, true, 1, 0, true>(tmA, tmB, p, stream);
-    if (BN == 192) {  // only chosen for the fast path (returned above) and the plain split-K accumulate path
-        if (cl2) return launch_gemm<192, 4, VTP_ACT_NONE, false, true, 1>(tmA, tmB, p, stream);
-        return launch_gemm<192, 4, VTP_ACT_NONE, false, false, 1>(tmA, tmB, p, stream);
-    }
     switch (a->act) {
         case VTP_ACT_NONE: VTP_LAUNCH(VTP_ACT_NONE, false);
         case VTP_ACT_GELU: VTP_LAUNCH(VTP_ACT_GELU, false);
-        case VTP_ACT_SWIGLU8: VTP_LAUNCH(VTP_ACT_SWIGLU8, false);
+        case VTP_ACT_SWIGLU8: return launch_gemm<128, 3, VTP_ACT_SWIGLU8, false>(tmA, tmB, p, stream);
         case VTP_ACT_ROPE: VTP_LAUNCH(VTP_ACT_ROPE, false);
         case VTP_ACT_RELU: VTP_LAUNCH(VTP_ACT_RELU, false);
         default: VTP_FAIL(VTP_ERR_ARG, "gemm: unknown activation %d", a->act);

@@ -15,7 +15,7 @@ int num_sms() {
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        if (n <= 0) n = 148;
+        if (n <= 0) n = 132;
     }
     return n;
 }
@@ -69,6 +69,7 @@ extern "C" int vtp_check_device(void) {
     cudaDeviceProp prop;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaGetDeviceProperties(&prop, dev) != cudaSuccess)
         VTP_FAIL(VTP_ERR_CUDA, "no CUDA device");
-    if (prop.major != 10) VTP_FAIL(VTP_ERR_ARCH, "device is sm_%d%d, this library is sm_100a only", prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0)
+        VTP_FAIL(VTP_ERR_ARCH, "device is sm_%d%d, this library is sm_90a only", prop.major, prop.minor);
     return VTP_OK;
 }

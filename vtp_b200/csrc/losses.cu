@@ -70,7 +70,7 @@ __device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
     return q;
 }
 
-// Round-2 rewrite (ncu, profiles/ncu_hbm_r2.md: 26 / 35 executed instructions per element, 25 % occupancy): 1024 threads per
+// Instruction- and occupancy-lean form: 1024 threads per
 // row block (32 warps/SM), base-2 exponentials with the temperature folded into one FFMA per element, every pass fully
 // vectorised on 16-byte shared / global accesses.
 __device__ __forceinline__ float ex2_approx(float x) {

@@ -1,5 +1,5 @@
 // vtp_b200 — LPIPS perceptual loss (utils/lpips.py:61-171) forward + gradient w.r.t. the reconstructed image.
-// The 13 VGG16 3x3 convolutions (and their dgrads) run on the tcgen05 GEMM in implicit-conv mode (gemm.cu, conv_C > 0);
+// The 13 VGG16 3x3 convolutions (and their dgrads) run on the wgmma GEMM in implicit-conv mode (gemm.cu, conv_C > 0);
 // this file holds the HBM-bound pieces around them, all on NHWC bf16 activations:
 //   lpips_prep      ScalingLayer (lpips.py:103-114) + im2col of the 3-channel input (K = 27 -> 32) for conv1_1
 //   maxpool2_fwd    nn.MaxPool2d(2,2)

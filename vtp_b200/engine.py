@@ -1,4 +1,4 @@
-"""Host orchestration of the sm_100a kernels: weight packing and tower forwards.
+"""Host orchestration of the sm_90a kernels: weight packing and tower forwards.
 
 Mirrors, stage by stage, the reference's L1/L2 code (vtp/models/layers/*, encoders/*, decoders/*) — every numeric op
 is a C-ABI kernel call from `lib`; torch is used for device memory (torch.empty) and integer index glue only.
@@ -7,7 +7,7 @@ Two precision modes, selected by the caller (VTPModel maps them from the autocas
   "bf16" — equals the reference under torch.autocast(bfloat16): bf16 GEMM/attention operands, fp32 accumulation,
            fp32 norms, fp32 residual stream in the encoder/text tower, bf16 stream in the decoder.
   "fp32" — equals the reference in fp32: every GEMM runs as a bf16x3 split (hi·hi + hi·lo + lo·hi, K-concatenated so
-           the same tcgen05 kernel is used; error ~2^-16), activations fp32, attention on fp32 CUDA cores.
+           the same wgmma kernel is used; error ~2^-16), activations fp32, attention on fp32 CUDA cores.
 """
 from __future__ import annotations
 
@@ -22,10 +22,10 @@ from .rope import rope_sincos
 BF = torch.bfloat16
 F32 = torch.float32
 # bf16 hot path: run the RoPE rotation and the SwiGLU gate as stand-alone full-occupancy kernels after a plain GEMM instead
-# of inside the GEMM epilogue (measured faster at K = 384: see csrc/elementwise.cu).  The fused epilogues stay available
+# of inside the GEMM epilogue (see csrc/elementwise.cu).  The fused epilogues stay available
 # (fp32 mode uses them; set False to use them in bf16 mode too — identical numerics, tests cover both).
 SPLIT_EPILOGUES = True
-# SwiGLU gate: the lean TMA-store epilogue variant of round 2 (csrc/gemm.cu fast_swiglu_tile) writes the hidden tensor
+# SwiGLU gate: the lean TMA-store epilogue variant (csrc/gemm.cu fast_swiglu_tile) writes the hidden tensor
 # (and, for training, the pre-activation) straight from the fc1 GEMM — no stand-alone gate pass re-reading [M, 2Hs].
 # VTP_FUSED_SWIGLU=0 restores the stand-alone swiglu_fwd kernel.
 import os as _os

@@ -1,4 +1,4 @@
-"""The consumer side of the encode/decode path (SURVEY.md §8f rank 2): the B200-native counterparts of
+"""The consumer side of the encode/decode path (SURVEY.md §8f rank 2): the H100-native counterparts of
 `generation/tokenizer/vtp_tokenizer.py` (class `VTP_Tokenizer`, same constructor arguments, attributes and methods) and
 of the latent-extraction loop of `generation/tools/extract_features_vtp.py` (same shard files, keys and metadata).
 

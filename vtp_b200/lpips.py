@@ -1,11 +1,11 @@
-"""LPIPS perceptual loss on the sm_100a kernels: value + gradient w.r.t. the reconstructed image.
+"""LPIPS perceptual loss on the sm_90a kernels: value + gradient w.r.t. the reconstructed image.
 
 Mirrors the reference's metric module vtp/utils/lpips.py:61-171 (ScalingLayer -> VGG16 features, 5 ReLU taps ->
 channel unit-normalise -> squared difference -> 1x1 `lin` -> spatial mean -> sum).  The reference downloads the VGG16 /
 lin weights at run time (lpips.py:15-17,48-58,130) which is impossible offline: weights are supplied by the caller
 (`from_tensors`) or drawn from a seeded generator (`random_init`, He-normal convs, positive lin weights) — SURVEY.md §7.
 
-All 13 3x3 convolutions and their input-gradients run on the tcgen05 GEMM in implicit-conv mode (4-D TMA over NHWC
+All 13 3x3 convolutions and their input-gradients run on the wgmma GEMM in implicit-conv mode (4-D TMA over NHWC
 bf16 activations, zero fill = padding; bias+ReLU, respectively the ReLU mask, fused in the epilogue); conv1_1 (3 input
 channels) goes through a 27->32 im2col.  Images are processed in chunks to bound activation memory.
 """

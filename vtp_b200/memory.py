@@ -1,12 +1,13 @@
 """HBM budget of the 3-objective training step (what `VTPTrainer` keeps resident), used to size the per-pass image
-groups (`TrainConfig.ssl_chunk / rec_chunk`) for the 180 GB of a B200.
+groups (`TrainConfig.ssl_chunk / rec_chunk`) for the 80 GB of an H100.
 
 The step saves, per token and per block, exactly what `engine.tower_blocks(..., tape=...)` appends:
     x_in, x_mid (residual stream: fp32 in the trunk / text tower, bf16 in the autocast decoder), h1, h2, o (bf16 [D]),
     qkv (bf16 [3D]), pre (bf16 [2·Hs] SwiGLU / [Hd] GELU), hid (bf16 [Hs] / [Hd]), lse + rstd (a few floats)
 => 20·D + 6·Hs bytes (fp32 stream, SwiGLU),  16·D + 6·Hs (bf16 stream),  20·D + 4·Hd (GELU MLP): `block_tape_bytes`.
 The three objectives run one after the other, so the peak is the largest single objective plus the persistent state.
-Calibration point (measured, profiles/bench_n2_r1.log): VTP-Small, 256 images/GPU, K = 65 536 -> 41.7 GiB peak.
+Calibration point (torch.cuda.max_memory_allocated on an H100, graph-captured step): VTP-Small, 256 images/GPU,
+K = 65 536 -> 42.7 GiB peak.
 """
 from __future__ import annotations
 
@@ -92,7 +93,7 @@ def train_step_bytes(cfg: VTPConfig, B: int, *, image: int = 256, local: int = 9
             "params": n["total"]}
 
 
-def suggest_chunks(cfg: VTPConfig, B: int, budget_bytes: float = 150 * GIB, **kw) -> Tuple[int, int]:
+def suggest_chunks(cfg: VTPConfig, B: int, budget_bytes: float = 64 * GIB, **kw) -> Tuple[int, int]:
     """Largest power-of-two-divided image groups (B, B/2, B/4, ...) whose estimated peak fits the budget.
     Returns (ssl_chunk, rec_chunk) with 0 = whole batch."""
     def fit(which: str) -> int:
@@ -111,3 +112,16 @@ def suggest_chunks(cfg: VTPConfig, B: int, budget_bytes: float = 150 * GIB, **kw
         raise ValueError("the contrastive objective cannot be split across passes and does not fit the budget; "
                          "lower the per-GPU batch")
     return fit("ssl"), fit("rec")
+
+
+def fit_batch(cfg: VTPConfig, B: int = 256, budget_bytes: float = 64 * GIB, **kw) -> int:
+    """Largest per-GPU batch B, B/2, B/4, ... for which `suggest_chunks` finds image groups that fit the budget (the
+    contrastive objective is not split, so it bounds the batch: VTP-Large runs 128 images per 80 GB GPU)."""
+    b = B
+    while b >= 1:
+        try:
+            suggest_chunks(cfg, b, budget_bytes, **kw)
+            return b
+        except ValueError:
+            b //= 2
+    raise ValueError(f"{cfg} does not fit {budget_bytes / GIB:.0f} GiB even one image per GPU")

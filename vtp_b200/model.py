@@ -1,5 +1,5 @@
 """VTPModel — the drop-in boundary (SURVEY.md §8b): same Python surface, attribute names and state-dict keys as
-the reference's vtp/models/vtp_hf/modeling_vtp.py:51-472, with every FLOP executed by the sm_100a kernels in
+the reference's vtp/models/vtp_hf/modeling_vtp.py:51-472, with every FLOP executed by the sm_90a kernels in
 libvtp_b200.so (see engine.py).  There is no eager/PyTorch fallback: on a CUDA-less host the API methods raise.
 
 Precision follows the caller's autocast context exactly like the reference does:
@@ -53,7 +53,7 @@ def check_head_dims(c: VTPConfig) -> None:
     for name, dim, heads in towers:
         if heads <= 0 or dim != 64 * heads:
             raise NotImplementedError(f"{name} tower: embed_dim {dim} / num_heads {heads} gives head_dim != 64; the "
-                                      "B200 attention kernels are specialised for head_dim == 64")
+                                      "the attention kernels are specialised for head_dim == 64")
 
 
 class _Holder(nn.Module):
@@ -108,9 +108,9 @@ class VTPModel(VTPPreTrainedModel):
         for flag, what in ((c.vision_init_values, "vision LayerScale"), (c.decoder_init_values, "decoder LayerScale"),
                            (c.text_ls_init_value, "text LayerScale")):
             if flag is not None:
-                raise NotImplementedError(f"{what} is not implemented by the B200 path (reference default is None)")
+                raise NotImplementedError(f"{what} is not implemented by the H100 path (reference default is None)")
         if c.vision_use_qk_norm or c.decoder_use_qk_norm:
-            raise NotImplementedError("qk-norm is not implemented by the B200 path (reference default is False)")
+            raise NotImplementedError("qk-norm is not implemented by the H100 path (reference default is False)")
         check_head_dims(c)
         self._init_vision_components()
         if c.train_clip:
@@ -214,7 +214,7 @@ class VTPModel(VTPPreTrainedModel):
         if c.text_embed_cls or c.text_no_causal_mask or c.text_pool_type != "argmax" or c.text_proj_bias or \
                 c.text_quick_gelu or c.text_proj_type != "linear":
             raise NotImplementedError("only the reference's default text tower (causal, argmax pool, GELU, linear "
-                                      "projection without bias) is implemented by the B200 path")
+                                      "projection without bias) is implemented by the H100 path")
         tt = _Holder()
         blocks = []
         for _ in range(c.text_depth):
@@ -371,7 +371,7 @@ class VTPModel(VTPPreTrainedModel):
             return hit[1]
         dev = self.trunk.cls_token.device
         if dev.type != "cuda":
-            raise lib.VtpError("VTPModel runs only on a CUDA (sm_100a) device; move the model with .cuda() — there is "
+            raise lib.VtpError("VTPModel runs only on a CUDA (sm_90a) device; move the model with .cuda() — there is "
                                "no CPU path")
         lib.check(lib.load().vtp_check_device(), "vtp_check_device")
         sd = {k: v for k, v in self.state_dict().items()}
@@ -454,7 +454,7 @@ class VTPModel(VTPPreTrainedModel):
         if self.config.vision_clip_feat == "cls":
             feat = out["x_norm_clstoken"]
         elif self.config.vision_clip_feat == "pooled":
-            raise NotImplementedError("vision_clip_feat='pooled' is not implemented by the B200 path")
+            raise NotImplementedError("vision_clip_feat='pooled' is not implemented by the H100 path")
         else:
             raise ValueError(f"Invalid vision_clip_feat: {self.config.vision_clip_feat}")
         B = feat.shape[0]

@@ -1,5 +1,5 @@
-"""The 3-objective training step (CLIP contrastive + DINO/iBOT self-distillation + pixel reconstruction) on the sm_100a
-kernels, with hand-written backward (no torch.autograd): the B200-native counterpart of the reference's legacy
+"""The 3-objective training step (CLIP contrastive + DINO/iBOT self-distillation + pixel reconstruction) on the sm_90a
+kernels, with hand-written backward (no torch.autograd): the H100-native counterpart of the reference's legacy
 meta-arch `VTP` (vtp/models/vtp.py:88-512: forward_clip / forward_ssl_learning / forward_reconstruction,
 update_teacher) plus the loss / optimiser layer that the reference does not release (SURVEY.md M3, a21).
 
@@ -296,9 +296,8 @@ class TrainConfig:
     rec_drop_rate: float = 0.0
     # collective C3: "end" = ONE all-reduce of the flat gradient buffer after the last backward; "overlap" = every tower's
     # bucket is all-reduced as soon as it is final, under the remaining backward (env VTP_GRAD_REDUCE overrides).
-    # Measured at N = 8 (profiles/r2_logs/bench_{small,large}_n8{,_end}.json): "end" 231.1 / 1317.5 ms vs "overlap"
-    # 233.6 / 1325.4 ms (Small / Large) — NCCL's CTAs take SMs away from the persistent, full-machine GEMM and attention
-    # kernels for longer than the ~1 ms (Small) / ~8 ms (Large, 3 GB fp32) the exposed all-reduce costs over NVLink.
+    # "end" is the default: overlapped collectives run NCCL's CTAs beside the persistent, full-machine GEMM and attention
+    # kernels and take SMs away from them for the whole backward.
     grad_reduce: str = "end"
 
 
