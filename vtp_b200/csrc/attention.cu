@@ -375,7 +375,8 @@ extern "C" int vtp_attention_fwd(const void* qkv, void* out, float* lse, int B, 
     VTP_CHECK_ARG(qkv && out && B > 0 && T > 0 && H > 0, "attention_fwd: bad args");
     VTP_CHECK_ARG(prefix >= 0 && prefix <= MAX_PREFIX && prefix < T, "attention_fwd: prefix must be in [0,%d]", MAX_PREFIX);
     const int HW = T - prefix;
-    VTP_CHECK_ARG(HW <= 256, "attention_fwd: %d non-prefix tokens > 256 is not supported by the single-pass kernel", HW);
+    VTP_CHECK_ARG(HW <= 256 || !causal, "attention_fwd: causal attention over %d > 256 non-prefix tokens is not supported",
+                  HW);
     VTP_CHECK_ARG(B <= 65535 && H <= 65535, "attention_fwd: grid too large");
     const int D = H * 64;
     AttnDev p;
@@ -395,6 +396,7 @@ extern "C" int vtp_attention_fwd(const void* qkv, void* out, float* lse, int B, 
     uint32_t box[2] = {64, 128};
     int rc = make_tmap_bf16(&tm, qkv, 2, dims, strides, box);
     if (rc) return rc;
+    if (HW > 256) return attn_fwd_long(tm, p, (cudaStream_t)st);  // the score row no longer fits one thread quad
     static bool configured = false;
     if (!configured) {
         VTP_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
@@ -412,7 +414,11 @@ extern "C" int vtp_attention_fwd_f32(const float* qkv, float* out, int B, int T,
     VTP_CHECK_ARG(qkv && out && B > 0 && T > 0 && H > 0 && B <= 65535, "attention_fwd_f32: bad args");
     const int nw = 8;
     const size_t smem = ((size_t)T * 65 + (size_t)T * 64 + (size_t)nw * T) * sizeof(float);
-    VTP_CHECK_ARG(smem <= 220 * 1024, "attention_fwd_f32: T=%d too long for the smem-resident kernel", T);
+    if (smem > 220 * 1024) {  // K/V no longer fit shared memory: stream them
+        VTP_CHECK_ARG(!causal, "attention_fwd_f32: causal attention over T=%d (beyond the smem-resident kernel) is not "
+                               "supported", T);
+        return attn_fwd_f32_tiled(qkv, out, B, T, H, (cudaStream_t)st);
+    }
     static size_t configured = 0;
     if (smem > configured) {
         VTP_CUDA(cudaFuncSetAttribute(attn_fwd_f32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

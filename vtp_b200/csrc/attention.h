@@ -18,4 +18,10 @@ struct AttnDev {
     float scale;
 };
 
+// attention_long.cu: non-causal forward for HW = T - prefix > 256 (streaming K/V, online softmax).  `tm` is the
+// tensor map of the packed qkv buffer with 64 x 128 boxes, as built by vtp_attention_fwd.
+int attn_fwd_long(const CUtensorMap& tm, const AttnDev& p, cudaStream_t st);
+// attention_long.cu: fp32 non-causal forward for T beyond the smem-resident attn_fwd_f32_kernel, K/V streamed in chunks
+int attn_fwd_f32_tiled(const float* qkv, float* out, int B, int T, int H, cudaStream_t st);
+
 }  // namespace vtp
