@@ -6,6 +6,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from tests.attn_ref import FWD_ROW_TOL, emulated_fwd, row_err
 from vtp_b200 import lib
 
 pytestmark = pytest.mark.gpu
@@ -111,7 +112,9 @@ def test_attention_fwd(B, T, H, prefix, causal, variant, monkeypatch):
     """attn_fwd_kernel<NKT>: one 128-key tile (HW <= 128) or two (128 < HW <= 256), cls / prefix rows on CUDA cores, causal
     text shapes, packed multi-sequence tiles for T <= 64 (VTP_ATTN_NO_PACK=1: one sequence per tile), with and without the
     saved log-sum-exp.  rows4 / rows8 / pipe are the ids of the three pre-Hopper forward kernels (one or two threads per
-    query row, persistent ping-pong); the Hopper build has the one kernel above, which all three ids run."""
+    query row, persistent ping-pong); the Hopper build has the one kernel above, which all three ids run.  The cls /
+    prefix rows, 1/T of the whole-tensor norm, are also checked row by row against the emulated bf16 reference
+    (tests/test_attention_rows_gpu.py checks every row)."""
     if variant == "VTP_ATTN_NO_PACK":
         monkeypatch.setenv(variant, "1")
     g = torch.Generator(device="cuda").manual_seed(B * 1000 + T)
@@ -123,6 +126,9 @@ def test_attention_fwd(B, T, H, prefix, causal, variant, monkeypatch):
     ref = _sdpa_ref(qkv, B, T, H, causal)
     assert torch.isfinite(out.float()).all()
     assert _rel(out, ref) < 6e-3, _rel(out, ref)
+    if prefix:
+        e = row_err(out, emulated_fwd(qkv, B, T, H, prefix, causal)[0], (B, T, 1, H))[:, :prefix].max().item()
+        assert e <= FWD_ROW_TOL, ("cls rows", e)
     if lse is None:
         return
     q, k, _ = [t.transpose(1, 2).float() for t in qkv.view(B, T, 3, H, 64).unbind(2)]
