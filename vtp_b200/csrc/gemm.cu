@@ -2,12 +2,13 @@
 //
 //   out[M,N] = epilogue( A[M,K] · B[N,K]ᵀ )      bf16 operands, fp32 accumulators
 //
-// Roles (384 threads): warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 = consumers.  BM = 128 (each consumer
-// warpgroup issues m64 wgmma for its 64 rows), BN in {64, 128}, BK = 64 bf16 = one 128B swizzle span, a STAGES-deep
-// TMA / mbarrier ring.  Operands may be K-major or MN-major (wgmma transpose bits), so forward (NT), dgrad (NN) and wgrad
-// (TN) all run through this one kernel; wgrad uses split-K + fp32 atomics.  After the mainloop the accumulators go
-// through a padded fp32 tile in shared memory, from which the eight consumer warps run the epilogue with one output row
-// per lane (32-row slabs); the producer meanwhile already streams the next tile's operands.
+// Roles (512 threads): warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 = MMA consumers, warpgroup 3 =
+// epilogue.  BM = 128 (each consumer warpgroup issues m64 wgmma for its 64 rows), BN in {64, 128}, BK = 64 bf16 = one 128B
+// swizzle span, a STAGES-deep TMA / mbarrier ring.  Operands may be K-major or MN-major (wgmma transpose bits), so forward
+// (NT), dgrad (NN) and wgrad (TN) all run through this one kernel; wgrad uses split-K + fp32 atomics.  After the mainloop
+// the consumers dump their accumulators into an fp32 tile in shared memory and go straight on to the next tile; the four
+// epilogue warps run the epilogue from that tile with one output row per lane (32-row slabs).  Two mbarriers hand the
+// tile over (acc_full: dumped, acc_empty: read), so the epilogue of tile t runs under the mainloop of tile t+1.
 //
 // Fused epilogues (all optional): +bias, bf16 rounding point, GELU, SwiGLU gate (8-interleaved w1|w2), axial
 // RoPE on q/k (bf16 arithmetic exactly as layers/attention.py:12-23,70-89), +residual, row remap (cls-token
@@ -22,7 +23,8 @@ namespace vtp {
 static constexpr int BM = 128;
 static constexpr int BK = 64;
 static constexpr int A_BYTES = BM * BK * 2;
-static constexpr int NUM_THREADS = 384;  // producer warpgroup + 2 consumer (MMA + epilogue) warpgroups
+static constexpr int NUM_THREADS = 512;  // producer warpgroup + 2 MMA consumer warpgroups + 1 epilogue warpgroup
+static constexpr int NUM_MMA_WARPS = 8;
 
 struct GemmDev {
     int M, N, K;
@@ -51,14 +53,14 @@ struct GemmDev {
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f)); }
 
 // ---------------------------------------------------------------------------------------------------- epilogue
-// 8 epilogue warps (the consumer warps).  Warp w owns row quarter (w & 3) of the tile and the 64-column units of
-// parity (w >> 2).  A unit is processed in two phases:
+// 4 epilogue warps.  Warp q owns row quarter q of the tile and all of its 64-column units.  A unit is processed in two
+// phases:
 //   A (row owner: lane = output row)  accumulator tile -> registers, +bias, rounding point, activation / RoPE
 //   B (cooperative)  the slab goes, 32 columns at a time, through a per-warp XOR-swizzled fp32 staging tile (4 KB) so
 //     that every global access is a contiguous 128-byte line per quarter-warp: residual read (prefetched into registers
 //     before the accumulator is even waited for), dtype conversion, store / red.add / PixelShuffle scatter.
 static constexpr int STG_FLOATS = 32 * 32;  // per epilogue warp
-static constexpr int NUM_EPI_WARPS = 8;
+static constexpr int NUM_EPI_WARPS = 4;
 
 __device__ __forceinline__ int stg_off(int r, int chunk /*0..7*/) { return r * 32 + ((chunk ^ (r & 7)) << 2); }
 
@@ -357,15 +359,42 @@ __device__ __forceinline__ void epilogue_unit(const GemmDev& p, float* stg, int 
 //   (mask_pos > 0) (ReLU backward of the LPIPS dgrads).   ACT: NONE | RELU.
 // Implicit-conv GEMMs (tile = conv_TH x conv_TW pixel patch of one image) store through a 4-D NHWC tensor map: the warp's
 // 32 rows are 32 / conv_TW image rows of conv_TW pixels.
-// 32 consecutive fp32 accumulator columns of this lane's row (the tile is padded: conflict-free 16-byte reads)
-__device__ __forceinline__ void acc_ld32(const float* arow, uint32_t (&r)[32]) {
+//
+// The fp32 accumulator tile acc_s holds BM rows of BN floats without padding; the 16-byte chunk k of row r sits at chunk
+// k ^ acc_key(r), acc_key(r) = 2 (r & 3) + ((r >> 2) & 1), which only permutes the low three chunk bits.  Bank groups of
+// 4 banks = 16-byte chunk index mod 8 (a row is a multiple of 128 bytes), and:
+//  - epilogue reads, 16 B per lane, lane = row: a quarter-warp reads one logical chunk of rows 8a .. 8a+7, and acc_key
+//    takes all 8 values on them, so the 8 reads fall into 8 distinct bank groups;
+//  - the wgmma fragment dump, 8 B per lane: a half-warp writes rows 8a + 4h + (0..3) (h = half-warp), logical chunks
+//    2j + ((lane >> 1) & 1) at 8-byte half (lane & 1).  The stored chunk's bits 2..1 are j ^ (r & 3) and bit 0 is
+//    ((lane >> 1) & 1) ^ h, so the 8 (row, chunk) pairs of a half-warp cover the 8 bank groups once and the 16 lanes the
+//    32 banks once.
+// (A +4-float row padding keeps the reads conflict-free but gives the dump 2-way conflicts.)
+__device__ __forceinline__ int acc_key(int r) { return ((r & 3) << 1) | ((r >> 2) & 1); }
+
+// 32 consecutive fp32 accumulator columns [col0, col0 + 32) of the lane's row (col0 % 32 == 0; key = acc_key(row))
+__device__ __forceinline__ void acc_ld32(const float* arow, int col0, int key, uint32_t (&r)[32]) {
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
-        const float4 v = *reinterpret_cast<const float4*>(arow + 4 * i);
+        const float4 v = *reinterpret_cast<const float4*>(arow + col0 + 4 * (i ^ key));
         r[4 * i] = __float_as_uint(v.x), r[4 * i + 1] = __float_as_uint(v.y), r[4 * i + 2] = __float_as_uint(v.z),
         r[4 * i + 3] = __float_as_uint(v.w);
     }
 }
+
+// Hand-off of acc_s from the MMA warps to the epilogue warps, one mbarrier phase per tile: acc_full completes when all
+// MMA warps have dumped the tile, acc_empty when all epilogue warps have read it (their stores may still be in flight).
+struct AccHandoff {
+    uint64_t* full;
+    uint64_t* empty;
+    uint32_t phase;  // parity of the current tile's phase
+    __device__ __forceinline__ void wait_full() const { mbar_wait(full, phase); }
+    // after this warp's last acc_s read of the tile
+    __device__ __forceinline__ void release(int lane) const {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty);
+    }
+};
 
 // Tile index t = work_id, work_id + stride, ... decomposed as t = (ks * num_m + m) * num_n + n WITHOUT a division per tile: the
 // producer is a single thread, and three runtime integer divisions per tile (~150 dependent instructions)
@@ -391,30 +420,30 @@ struct TileIter {
 
 // ---- SwiGLU gate in the lean epilogue (FAST 6: hidden + pre-activation outputs, FAST 7: hidden only).
 // The stand-alone gate pass re-read the whole [M, 2Hs] pre-activation (539 MB per FFN forward at the bench shape, 6.6 ms of
-// the step); here the epilogue warp that owns two ADJACENT 64-column packed chunks (8-interleaved w1|w2: columns
-// [16g, 16g+8) = x1, [16g+8, 16g+16) = x2) stores them as the pre-activation through tmO2 and writes their 32 + 32 hidden
-// values  round(round(silu(x1)) * x2)  (layers/ffn.py:77-81 under autocast) into a second 32 x 128-byte staging tile that
-// leaves through ONE TMA store of the [M, Hs] hidden tensor (tmO).
+// the step); here the epilogue warp takes the two ADJACENT 64-column packed chunks of its rows (8-interleaved w1|w2:
+// columns [16g, 16g+8) = x1, [16g+8, 16g+16) = x2), stores them as the pre-activation through tmO2 and writes their 32 + 32
+// hidden values  round(round(silu(x1)) * x2)  (layers/ffn.py:77-81 under autocast) into a second 32 x 128-byte staging tile
+// that leaves through ONE TMA store of the [M, Hs] hidden tensor (tmO).
 template <int BN, int FAST>
 __device__ __forceinline__ void fast_swiglu_tile(const GemmDev& p, const CUtensorMap* tmO, const CUtensorMap* tmO2, uint8_t* stg,
-                                                 uint8_t* stg2, float* bias_s, int lane, int q, int hsel, const float* arow,
-                                                 int m_blk, int n0) {
+                                                 uint8_t* stg2, float* bias_s, int lane, int q, const AccHandoff& ah,
+                                                 const float* arow, int key, int m_blk, int n0) {
+    static_assert(BN == 128, "one packed chunk pair = one 64-column hidden line per tile row");
     constexpr bool PRE = FAST == 6;
-    constexpr int TCH = BN / 64;             // packed 64-column chunks per tile row (BN in {128, 256})
     const int m0 = m_blk * BM;
     const int N = p.N;
-    const int c0 = 2 * hsel;                 // this warp's chunk pair (2 hsel, 2 hsel + 1) -> hidden columns [64 hsel, +64)
-    const bool have = c0 < TCH && n0 + c0 * 64 < N;
-    if (have) {
+    ah.wait_full();
+    {
 #pragma unroll
         for (int j = 0; j < 2; ++j) {
-            const int col0 = n0 + (c0 + j) * 64;
+            const int col0 = n0 + j * 64;
             const bool valid = col0 < N;     // warp-uniform (ragged last tile: N % 64 != 0 is clipped by the tensor maps)
             uint32_t r0[32], r1[32];
             if (valid) {
-                acc_ld32(arow + (c0 + j) * 64, r0);
-                acc_ld32(arow + (c0 + j) * 64 + 32, r1);
+                acc_ld32(arow, j * 64, key, r0);
+                acc_ld32(arow, j * 64 + 32, key, r1);
             }
+            if (j == 1) ah.release(lane);
             bias_s[lane] = (p.bias && col0 + lane < N) ? __ldg(p.bias + col0 + lane) : 0.f;
             bias_s[32 + lane] = (p.bias && col0 + 32 + lane < N) ? __ldg(p.bias + col0 + 32 + lane) : 0.f;
             if (lane == 0) bulk_wait_read0();   // earlier TMA stores of this warp have finished reading both staging tiles
@@ -463,7 +492,7 @@ __device__ __forceinline__ void fast_swiglu_tile(const GemmDev& p, const CUtenso
         fence_proxy_async_smem();
         __syncwarp();
         if (lane == 0) {
-            tma_store_2d(tmO, stg2, (n0 >> 1) + 64 * hsel, m0 + q * 32);
+            tma_store_2d(tmO, stg2, n0 >> 1, m0 + q * 32);
             bulk_commit();
         }
     }
@@ -471,14 +500,14 @@ __device__ __forceinline__ void fast_swiglu_tile(const GemmDev& p, const CUtenso
 
 template <int BN, int ACT, int FAST>
 __device__ __forceinline__ void fast_epilogue_tile(const GemmDev& p, const CUtensorMap* tmO, uint8_t* stg, float* bias_s,
-                                                   int lane, int q, int hsel, const float* arow, int m_blk, int n0) {
+                                                   int lane, int q, const AccHandoff& ah, const float* arow, int key,
+                                                   int m_blk, int n0) {
     constexpr bool OF32 = FAST == 3 || FAST == 4;
     constexpr bool MASK = FAST == 5;
     constexpr bool RES = FAST == 2 || FAST == 4 || MASK;  // a second [M][N]-shaped operand read one chunk ahead
     const int m0 = m_blk * BM;
     constexpr int CW = OF32 ? 32 : 64;   // accumulator columns per 128-byte output chunk
-    constexpr int TCH = BN / CW;         // chunks per tile row
-    constexpr int NCH = (TCH + 1) / 2;   // chunks per warp and tile (the two warps of a lane quarter interleave)
+    constexpr int TCH = BN / CW;         // chunks per tile row, all taken by this warp
     constexpr int PW = OF32 ? 4 : 8;     // columns per 16-byte piece
     const int N = p.N;
     long row = (long)m0 + q * 32 + lane;
@@ -512,28 +541,27 @@ __device__ __forceinline__ void fast_epilogue_tile(const GemmDev& p, const CUten
                                               : make_uint4(0, 0, 0, 0);
         }
     };
-    if (n0 + hsel * CW < N) {
-        load_bias(n0 + hsel * CW);
-        if (RES) {
-            load_resid(n0 + hsel * CW);  // first chunk: in registers before the accumulator is waited for
+    load_bias(n0);
+    if (RES) {
+        load_resid(n0);  // first chunk: in registers before the accumulator is waited for
 #pragma unroll
-            for (int j = 1; j < NCH; ++j) {  // later chunks: warm this lane's 128-byte row piece in L2
-                const int col = n0 + (hsel + 2 * j) * CW;
-                if (row_ok && col < N && hsel + 2 * j < TCH) asm volatile("prefetch.global.L2 [%0];" ::"l"(rrow + (long)col * (OF32 ? 4 : 2)));
-            }
+        for (int j = 1; j < TCH; ++j) {  // later chunks: warm this lane's 128-byte row piece in L2
+            const int col = n0 + j * CW;
+            if (row_ok && col < N) asm volatile("prefetch.global.L2 [%0];" ::"l"(rrow + (long)col * (OF32 ? 4 : 2)));
         }
     }
+    ah.wait_full();
 #pragma unroll
-    for (int j = 0; j < NCH; ++j) {
-        const int c = hsel + 2 * j;
+    for (int c = 0; c < TCH; ++c) {
         const int col0 = n0 + c * CW;
-        if (c >= TCH || col0 >= N) break;  // warp-uniform
-        const bool last = (j == NCH - 1) || (c + 2 >= TCH) || (col0 + 2 * CW >= N);
+        if (col0 >= N) break;  // warp-uniform
+        const bool last = (c == TCH - 1) || (col0 + CW >= N);
         const float b0 = b0n, b1 = b1n;
-        if (!last) load_bias(col0 + 2 * CW);
+        if (!last) load_bias(col0 + CW);
         uint32_t r0[32], r1[32];
-        acc_ld32(arow + c * CW, r0);
-        if (!OF32) acc_ld32(arow + c * CW + 32, r1);
+        acc_ld32(arow, c * CW, key, r0);
+        if (!OF32) acc_ld32(arow, c * CW + 32, key, r1);
+        if (last) ah.release(lane);
         bias_s[lane] = b0;
         if (!OF32) bias_s[32 + lane] = b1;
         if (lane == 0) bulk_wait_read0();  // the previous TMA store has finished reading the staging tile
@@ -579,7 +607,7 @@ __device__ __forceinline__ void fast_epilogue_tile(const GemmDev& p, const CUten
                     *reinterpret_cast<uint4*>(stg + stgb_off(lane, i)) = w;
                 }
             }
-            if (RES && !last) load_resid(col0 + 2 * CW);  // in flight across the store and the next accumulator read
+            if (RES && !last) load_resid(col0 + CW);  // in flight across the store and the next accumulator read
             fence_proxy_async_smem();
             __syncwarp();
             if (lane == 0) {
@@ -630,16 +658,17 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     static_assert(BN == 64 || BN == 128, "tile width");
     constexpr int B_BYTES = BN * BK * 2;
     constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    constexpr int ACC_LD = BN + 4;  // padded fp32 accumulator rows
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     constexpr int STG_BYTES = NUM_EPI_WARPS * STG_FLOATS * 4 * (FAST == 6 ? 2 : 1);  // FAST 6: + the hidden-tile staging
     uint8_t* ring = smem;
     float* acc_s = reinterpret_cast<float*>(ring + STAGES * STAGE_BYTES);
-    float* stg_base = acc_s + BM * ACC_LD;                                                 // 8 epilogue warps x 4 KB
+    float* stg_base = acc_s + BM * BN;                                                     // 4 epilogue warps x 4 KB
     float* bias_base = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(stg_base) + STG_BYTES);  // FAST only
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(bias_base) + (FAST ? NUM_EPI_WARPS * 256 : 0));
     uint64_t* empty_bar = full_bar + STAGES;
+    uint64_t* acc_full = empty_bar + STAGES;
+    uint64_t* acc_empty = acc_full + 1;
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -651,14 +680,16 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         tma_prefetch_desc(&tmB);
         if (FAST) tma_prefetch_desc(&tmO);
         if (FAST == 6) tma_prefetch_desc(&tmO2);
-        for (int s = 0; s < STAGES; ++s) mbar_init(&full_bar[s], 1), mbar_init(&empty_bar[s], NUM_EPI_WARPS);
+        for (int s = 0; s < STAGES; ++s) mbar_init(&full_bar[s], 1), mbar_init(&empty_bar[s], NUM_MMA_WARPS);
+        mbar_init(acc_full, NUM_MMA_WARPS);
+        mbar_init(acc_empty, NUM_EPI_WARPS);
         fence_barrier_init();
     }
     __syncthreads();
 
-    const int tiles_mn = p.num_m_blocks * p.num_n_blocks;
-    const int num_tiles = tiles_mn * p.num_splits;
-
+    const int num_tiles = p.num_m_blocks * p.num_n_blocks * p.num_splits;
+    // registers per thread: producer 40, MMA 144, epilogue 184 (40 + 2 * 144 + 184 = 4 * 128: the 64K register file).
+    // ptxas allocates each role within its setmaxnreg count; this split compiles every instantiation without spills.
     if (warp < 4) {
         // ============================== TMA producer ==============================
         setmaxnreg_dec<40>();
@@ -712,22 +743,16 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                 }
             }
         }
-    } else {
-        // ============================== consumers: wgmma mainloop, then the epilogue ==============================
-        setmaxnreg_inc<232>();
+    } else if (warp < 4 + NUM_MMA_WARPS) {
+        // ============================== MMA consumers: wgmma mainloop, accumulator dump ==============================
+        setmaxnreg_inc<144>();
         const int wg = (warp >> 2) - 1;    // consumer warpgroup: tile rows [64 wg, 64 wg + 64)
-        const int q = warp & 3;            // row quarter of the tile this warp runs the epilogue for
-        const int hsel = (warp - 4) >> 2;  // parity of the 64-column units this warp handles
         const int tw = threadIdx.x & 127;
-        float* stg = stg_base + (warp - 4) * STG_FLOATS;
-        const bool has_resid = p.resid != nullptr;
-        const float* arow = acc_s + (q * 32 + lane) * ACC_LD;
         int s = 0;
-        uint32_t ph = 0;
+        uint32_t ph = 0, acc_ph = 0;
         TileIter ti(work_id, work_stride, p.num_n_blocks, p.num_m_blocks);
         for (int t = work_id; t < num_tiles; t += work_stride, ti.next()) {
-            const int n_blk = ti.n, m_blk = ti.m, ks = ti.ks;
-            const int kb0 = ks * p.kb_per_split;
+            const int kb0 = ti.ks * p.kb_per_split;
             const int nkb = min(kb0 + p.kb_per_split, p.num_k_blocks) - kb0;
             float acc[BN / 2];
             if (p.a_mn) {
@@ -737,49 +762,65 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                 if (p.b_mn) gemm_mainloop<BN, STAGES, 0, 1>(acc, ring, full_bar, empty_bar, s, ph, nkb, wg, lane);
                 else gemm_mainloop<BN, STAGES, 0, 0>(acc, ring, full_bar, empty_bar, s, ph, nkb, wg, lane);
             }
-            // accumulators -> padded fp32 tile (the previous tile's epilogue has finished reading it)
-            asm volatile("bar.sync 1, 256;" ::: "memory");
+            // accumulators -> swizzled fp32 tile, once the epilogue warps have read the previous tile out of it
+            mbar_wait(acc_empty, acc_ph ^ 1);
             {
                 const int r0 = 64 * wg + 16 * (tw >> 5) + ((tw & 31) >> 2), c0 = 2 * (tw & 3);
+                const int key = acc_key(r0);  // rows r0 and r0 + 8 share it
 #pragma unroll
                 for (int j = 0; j < BN / 8; ++j) {
-                    *reinterpret_cast<float2*>(acc_s + r0 * ACC_LD + 8 * j + c0) = make_float2(acc[4 * j], acc[4 * j + 1]);
-                    *reinterpret_cast<float2*>(acc_s + (r0 + 8) * ACC_LD + 8 * j + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+                    const int off = 4 * ((2 * j + (c0 >> 2)) ^ key) + (c0 & 3);
+                    *reinterpret_cast<float2*>(acc_s + r0 * BN + off) = make_float2(acc[4 * j], acc[4 * j + 1]);
+                    *reinterpret_cast<float2*>(acc_s + (r0 + 8) * BN + off) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
                 }
             }
-            asm volatile("bar.sync 1, 256;" ::: "memory");
-            const int m0 = m_blk * BM, n0 = n_blk * BN;
+            __syncwarp();
+            if (lane == 0) mbar_arrive(acc_full);
+            acc_ph ^= 1;
+        }
+    } else {
+        // ============================== epilogue warps ==============================
+        setmaxnreg_inc<184>();
+        const int q = warp & 3;  // row quarter of the tile: rows [32 q, 32 q + 32), lane = row
+        float* stg = stg_base + q * STG_FLOATS;
+        const bool has_resid = p.resid != nullptr;
+        const float* arow = acc_s + (q * 32 + lane) * BN;
+        const int key = acc_key(lane);
+        AccHandoff ah{acc_full, acc_empty, 0};
+        TileIter ti(work_id, work_stride, p.num_n_blocks, p.num_m_blocks);
+        for (int t = work_id; t < num_tiles; t += work_stride, ti.next(), ah.phase ^= 1) {
+            const int m_blk = ti.m, n0 = ti.n * BN;
+            const int m0 = m_blk * BM;
             const int grow0 = m0 + q * 32;
             if constexpr (FAST == 6 || FAST == 7) {
                 uint8_t* st1 = reinterpret_cast<uint8_t*>(stg);
-                // FAST 6: second tile behind the eight pre-activation tiles; FAST 7: the only tile holds the hidden values
-                uint8_t* st2 = FAST == 6 ? reinterpret_cast<uint8_t*>(stg_base) + (NUM_EPI_WARPS + (warp - 4)) * STG_FLOATS * 4 : st1;
-                fast_swiglu_tile<BN, FAST>(p, &tmO, &tmO2, st1, st2, bias_base + (warp - 4) * 64, lane, q, hsel, arow, m_blk, n0);
+                // FAST 6: second tile behind the pre-activation tiles; FAST 7: the only tile holds the hidden values
+                uint8_t* st2 = FAST == 6 ? reinterpret_cast<uint8_t*>(stg_base) + (NUM_EPI_WARPS + q) * STG_FLOATS * 4 : st1;
+                fast_swiglu_tile<BN, FAST>(p, &tmO, &tmO2, st1, st2, bias_base + q * 64, lane, q, ah, arow, key, m_blk, n0);
                 continue;
             }
             if constexpr (FAST != 0) {
-                fast_epilogue_tile<BN, ACT, FAST>(p, &tmO, reinterpret_cast<uint8_t*>(stg), bias_base + (warp - 4) * 64, lane, q,
-                                                  hsel, arow, m_blk, n0);
+                fast_epilogue_tile<BN, ACT, FAST>(p, &tmO, reinterpret_cast<uint8_t*>(stg), bias_base + q * 64, lane, q, ah,
+                                                  arow, key, m_blk, n0);
                 continue;
             }
             constexpr bool sw = ACT == VTP_ACT_SWIGLU8;
             long orow8[8];  // output rows of the cooperative store pattern (row 4*it + lane/8 of this warp's slab)
 #pragma unroll
             for (int it = 0; it < 8; ++it) orow8[it] = out_row(p, grow0 + 4 * it + (lane >> 3));
-            // unit assignment: parity-interleaved, except SwiGLU where a warp takes ADJACENT packed units (2k, 2k+1) so
-            // that their 32+32 hidden columns form one full 128-byte output line
+            // units in order: for SwiGLU the packed units (2k, 2k+1) form one full 128-byte hidden output line
             uint32_t hold[16];  // first half of a SwiGLU hidden line, kept in registers until its partner unit is done
+            ah.wait_full();
 #pragma unroll 1
-            for (int j = 0; j < BN / 64; ++j) {
-                const int u = sw ? (hsel == 0 ? j : BN / 64) : hsel + 2 * j;
-                if (u >= BN / 64) break;
+            for (int u = 0; u < BN / 64; ++u) {
                 const int col0 = n0 + u * 64;
                 if (col0 >= p.N) break;  // warp-uniform
                 if (has_resid)  // pull the residual lines into L2 before they are read
                     prefetch_resid_l2(p, lane, orow8, sw ? col0 >> 1 : col0, sw ? 32 : 64, sw ? p.N >> 1 : p.N);
                 uint32_t r0[32], r1[32];
-                acc_ld32(arow + u * 64, r0);
-                acc_ld32(arow + u * 64 + 32, r1);
+                acc_ld32(arow, u * 64, key, r0);
+                acc_ld32(arow, u * 64 + 32, key, r1);
+                if (u == BN / 64 - 1 || col0 + 64 >= p.N) ah.release(lane);
                 float v[64];
 #pragma unroll
                 for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r0[i]), v[32 + i] = __uint_as_float(r1[i]);
@@ -793,9 +834,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 template <int BN, int STAGES, int ACT, bool PS, int FAST = 0>
 static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& p, cudaStream_t stream,
                        const CUtensorMap* tmO = nullptr, const CUtensorMap* tmO2 = nullptr) {
-    constexpr int smem_bytes = 1024 + STAGES * (A_BYTES + BN * BK * 2) + BM * (BN + 4) * 4 +
+    constexpr int smem_bytes = 1024 + STAGES * (A_BYTES + BN * BK * 2) + BM * BN * 4 +
                                NUM_EPI_WARPS * STG_FLOATS * 4 * (FAST == 6 ? 2 : 1) + (FAST ? NUM_EPI_WARPS * 256 : 0) +
-                               2 * STAGES * 8;
+                               (2 * STAGES + 2) * 8;
     static_assert(smem_bytes <= 232448, "shared memory budget (227 KB per block)");
     static bool configured = false;
     if (!configured) {
