@@ -138,10 +138,18 @@ int vtp_attention_fwd_f32(const float* qkv, float* out, int B, int T, int H, int
  * Training step (the reference releases no training loop — SURVEY.md M3/a21; these are the autograd duals of the
  * forward stages above plus restated losses and a fused optimiser)
  * ------------------------------------------------------------------------------------------------------------ */
-/* dual of vtp_attention_fwd incl. the RoPE rotation (layers/attention.py:70-89,110-126): dqkv = d/d(pre-RoPE qkv) */
+/* dual of vtp_attention_fwd incl. the RoPE rotation (layers/attention.py:70-89,110-126): dqkv = d/d(pre-RoPE qkv).
+ * Single pass, the whole sequence in one CTA: HW = T - prefix <= 256 (VTP_ERR_ARG above; see vtp_attention_bwd_long) */
 int vtp_attention_bwd(const void* qkv, const void* o, const void* dout, const float* lse, void* dqkv,
                       const void* rope_sin, const void* rope_cos, int B, int T, int H, int prefix, int causal,
                       vtp_stream_t stream);
+/* same op, non-causal, for any HW = T - prefix >= 1 (layers/attention.py:70-89,110-126 at image sizes above 256x256;
+ * attention_bwd_long.cu): K/V and Q/dO stream through shared memory instead of one CTA holding the sequence.  prefix
+ * 0 or 1.  delta_ws: fp32 workspace [B][H][T] (like lse), overwritten with δ = Σ dO·O.  No atomics: repeat launches
+ * are bit-identical. */
+int vtp_attention_bwd_long(const void* qkv, const void* o, const void* dout, const float* lse, float* delta_ws,
+                           void* dqkv, const void* rope_sin, const void* rope_cos, int B, int T, int H, int prefix,
+                           vtp_stream_t stream);
 /* dual of vtp_norm_fwd: g[M][D] (fp32 stream gradient) += dx ; dw[D] += ; db[D] += (LayerNorm).  Optional fused
  * by-products of the updated g: g_bf16_out [M][D] (the dY operand of the preceding sub-layer) and g_colsum[D] += Σ_m g
  * (that sub-layer's bias gradient) */

@@ -11,6 +11,7 @@
 // threads (rank-1 updates + a column reduction for dK_0/dV_0) and as an extra query row by a spare warp.
 #include <stdlib.h>
 
+#include "attention_bwd.cuh"
 #include "host.h"
 #include "ptx.cuh"
 
@@ -37,31 +38,6 @@ struct AttnBwdDev {
     int pack, rprefix;
 };
 
-__device__ __forceinline__ float ex2f(float x) {  // ex2.approx.ftz: no denormal slow path (exp2f() costs 4 extra instr)
-    float y;
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-    return y;
-}
-__device__ __forceinline__ uint32_t sw_off(int row, int col) {
-    return row * 128 + ((((col >> 3) ^ (row & 7)) << 4) | ((col & 7) << 1));
-}
-__device__ __forceinline__ void load_row64(const uint8_t* tile, int row, float (&f)[64]) {
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-        const uint4 w = *reinterpret_cast<const uint4*>(tile + sw_off(row, c * 8));
-        f[c * 8 + 0] = bf16_lo(w.x), f[c * 8 + 1] = bf16_hi(w.x), f[c * 8 + 2] = bf16_lo(w.y), f[c * 8 + 3] = bf16_hi(w.y);
-        f[c * 8 + 4] = bf16_lo(w.z), f[c * 8 + 5] = bf16_hi(w.z), f[c * 8 + 6] = bf16_lo(w.w), f[c * 8 + 7] = bf16_hi(w.w);
-    }
-}
-__device__ __forceinline__ void load_grow64(const __nv_bfloat16* g, float (&f)[64]) {
-    const uint4* p = reinterpret_cast<const uint4*>(g);
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-        const uint4 w = __ldg(p + c);
-        f[c * 8 + 0] = bf16_lo(w.x), f[c * 8 + 1] = bf16_hi(w.x), f[c * 8 + 2] = bf16_lo(w.y), f[c * 8 + 3] = bf16_hi(w.y);
-        f[c * 8 + 4] = bf16_lo(w.z), f[c * 8 + 5] = bf16_hi(w.z), f[c * 8 + 6] = bf16_lo(w.w), f[c * 8 + 7] = bf16_hi(w.w);
-    }
-}
 __device__ __forceinline__ void store_row64(__nv_bfloat16* g, const float (&f)[64]) {
     uint4* p = reinterpret_cast<uint4*>(g);
 #pragma unroll
@@ -82,27 +58,6 @@ __device__ __forceinline__ void rope_bwd64(float (&g)[64], const __nv_bfloat16* 
         const float a = g[i], b = g[i + 32];
         g[i] = a * cs[i] + b * sn[i + 32];
         g[i + 32] = b * cs[i + 32] - a * sn[i];
-    }
-}
-
-// RoPEᵀ on the 16 dims of a row that a thread of the quad holds in an m64n64 accumulator fragment: g[2 jn + c] is dim
-// 8 jn + 2 c4 + c, so dims d and d + 32 (jn and jn + 4) sit in the same thread
-__device__ __forceinline__ void rope_bwd_frag(float (&g)[16], const __nv_bfloat16* sin_row, const __nv_bfloat16* cos_row, int c4) {
-#pragma unroll
-    for (int jn = 0; jn < 4; ++jn) {
-        const int d = 8 * jn + 2 * c4;
-        const uint32_t s_lo = __ldg(reinterpret_cast<const uint32_t*>(sin_row + d));
-        const uint32_t s_hi = __ldg(reinterpret_cast<const uint32_t*>(sin_row + d + 32));
-        const uint32_t c_lo = __ldg(reinterpret_cast<const uint32_t*>(cos_row + d));
-        const uint32_t c_hi = __ldg(reinterpret_cast<const uint32_t*>(cos_row + d + 32));
-        const float sl[2] = {bf16_lo(s_lo), bf16_hi(s_lo)}, sh[2] = {bf16_lo(s_hi), bf16_hi(s_hi)};
-        const float cl[2] = {bf16_lo(c_lo), bf16_hi(c_lo)}, ch[2] = {bf16_lo(c_hi), bf16_hi(c_hi)};
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-            const float a = g[2 * jn + c], b = g[2 * (jn + 4) + c];
-            g[2 * jn + c] = a * cl[c] + b * sh[c];
-            g[2 * (jn + 4) + c] = b * ch[c] - a * sl[c];
-        }
     }
 }
 
@@ -156,21 +111,6 @@ __global__ void __launch_bounds__(AB_THREADS, 1) attn_bwd_kernel(const __grid_co
         const __nv_bfloat16* vcls = p.qkv + row0 * 3 * D + 2 * D + h * 64;
         float lse_i[NKT][2], delta_i[NKT][2], ds_own[NKT][2];
         float dv[32], dk[32], dq[NKT][32];
-        // quad-split 64-dim dot product of two bf16 rows (16 dims per thread of the quad), summed over the quad
-        auto dot_quad = [&](const uint8_t* tile, int row, const __nv_bfloat16* g) {
-            float acc = 0.f;
-#pragma unroll
-            for (int c = 0; c < 2; ++c) {
-                const uint4 a = *reinterpret_cast<const uint4*>(tile + sw_off(row, 16 * c4 + 8 * c));
-                const uint4 w = __ldg(reinterpret_cast<const uint4*>(g + 16 * c4 + 8 * c));
-                const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, ww[4] = {w.x, w.y, w.z, w.w};
-#pragma unroll
-                for (int e = 0; e < 4; ++e) acc += bf16_lo(aw[e]) * bf16_lo(ww[e]) + bf16_hi(aw[e]) * bf16_hi(ww[e]);
-            }
-            acc += __shfl_xor_sync(0xffffffffu, acc, 1);
-            acc += __shfl_xor_sync(0xffffffffu, acc, 2);
-            return acc;
-        };
 
 #pragma unroll
         for (int n = 0; n < NKT * NKT; ++n) {
@@ -186,15 +126,15 @@ __global__ void __launch_bounds__(AB_THREADS, 1) attn_bwd_kernel(const __grid_co
                     lse_i[t][i] = 0.f, delta_i[t][i] = 0.f, ds_own[t][i] = 0.f;
                     float p0v = 0.f, ds0v = 0.f;
                     if (__any_sync(0xffffffffu, qvalid)) {  // quads are uniform: the shuffles stay inside valid quads
-                        const float dl = dot_quad(smem + BDO + t * 16384, rr[i], p.o + (qvalid ? grow : row0) * D + h * 64);
+                        const float dl = quad_dot(smem + BDO + t * 16384, rr[i], p.o + (qvalid ? grow : row0) * D + h * 64, c4);
                         if (qvalid) {
                             lse_i[t][i] = p.pack ? p.lse[((long)(b + pseq[i]) * p.H + h) * T + ptok[i]]
                                                  : p.lse[((long)b * p.H + h) * T + prefix + qi];
                             delta_i[t][i] = dl;
                         }
                         if (prefix > 0) {
-                            const float dp0 = dot_quad(smem + BDO + t * 16384, rr[i], vcls);
-                            const float s0 = dot_quad(smem + BQ + t * 16384, rr[i], kcls);
+                            const float dp0 = quad_dot(smem + BDO + t * 16384, rr[i], vcls, c4);
+                            const float s0 = quad_dot(smem + BQ + t * 16384, rr[i], kcls, c4);
                             if (qvalid) {
                                 p0v = ex2f(s0 * p.scale_log2 - lse_i[t][i] * lse_l2);
                                 ds0v = p.scale * p0v * (dp0 - dl);

@@ -72,6 +72,7 @@ SIGNATURES: dict[str, tuple] = {
                                     C.c_void_p]),
     "vtp_attention_fwd_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "vtp_attention_bwd": (C.c_int, [C.c_void_p] * 7 + [C.c_int] * 5 + [C.c_void_p]),
+    "vtp_attention_bwd_long": (C.c_int, [C.c_void_p] * 8 + [C.c_int] * 4 + [C.c_void_p]),
     "vtp_norm_bwd": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vtp_swiglu_bwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
@@ -300,6 +301,14 @@ def attention_bwd(qkv, o, dout, lse, dqkv, B: int, T: int, H: int, *, prefix: in
     sin, cos = (rope[0], rope[1]) if rope is not None else (None, None)
     check(load().vtp_attention_bwd(_ptr(qkv), _ptr(o), _ptr(dout), _ptr(lse), _ptr(dqkv), _ptr(sin), _ptr(cos), B, T, H,
                                    prefix, int(causal), _st(stream)), "vtp_attention_bwd")
+
+
+def attention_bwd_long(qkv, o, dout, lse, delta, dqkv, B: int, T: int, H: int, *, prefix: int, rope=None, stream=None):
+    """Non-causal attention backward for any length; delta: fp32 workspace [B, H, T] (overwritten)."""
+    _check_qkv(qkv, B, T, H)
+    sin, cos = (rope[0], rope[1]) if rope is not None else (None, None)
+    check(load().vtp_attention_bwd_long(_ptr(qkv), _ptr(o), _ptr(dout), _ptr(lse), _ptr(delta), _ptr(dqkv), _ptr(sin),
+                                        _ptr(cos), B, T, H, prefix, _st(stream)), "vtp_attention_bwd_long")
 
 
 def norm_bwd(x, rstd, mean, w, dy, g, dw, db, M: int, D: int, gb_out=None, g_colsum=None, stream=None):

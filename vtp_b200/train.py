@@ -139,6 +139,18 @@ def dgrad(dy: torch.Tensor, w: torch.Tensor, out: torch.Tensor, Mtok: int, **kw)
     lib.gemm(dy, w, out, M=Mtok, N=k_in, K=n_out, b_mn=True, lda=dy.stride(0), ldb=k_in, round_bf16=False, **kw)
 
 
+def attention_backward(t: dict, do: torch.Tensor, dqkv: torch.Tensor, B: int, T: int, H: int, prefix: int, causal: bool,
+                       rope):
+    """dqkv = d/d(pre-RoPE qkv) of one attention sub-layer from its tape entry t (qkv, o, lse).  Up to 256 patch tokens
+    the single-pass kernel holds the whole sequence in one CTA; longer non-causal sequences (images above 256x256) go
+    to the streaming kernels, which need an fp32 workspace for δ = Σ dO·O laid out like lse."""
+    if T - prefix > 256 and not causal:
+        delta = _e((B, H, T), F32, do.device)
+        lib.attention_bwd_long(t["qkv"], t["o"], do, t["lse"], delta, dqkv, B, T, H, prefix=prefix, rope=rope)
+    else:
+        lib.attention_bwd(t["qkv"], t["o"], do, t["lse"], dqkv, B, T, H, prefix=prefix, causal=causal, rope=rope)
+
+
 def tower_blocks_backward(W: TowerW, G: TowerW, tape: list, g: torch.Tensor, B: int, T: int, rope, causal=False):
     """Reverse of engine.tower_blocks.  g fp32 [B*T, D]: in = dL/d(stream out), out = dL/d(stream in) (in place).
     The bf16 copy of g (dY operand of the next sub-layer to differentiate) and its column sums (that sub-layer's bias
@@ -172,7 +184,7 @@ def tower_blocks_backward(W: TowerW, G: TowerW, tape: list, g: torch.Tensor, B: 
         dgrad(gb, bw.proj.w, do, M)
         wgrad(gb, t["o"], gw.proj.w, M)
         dqkv = _e((M, 3 * D), BF, dev)
-        lib.attention_bwd(t["qkv"], t["o"], do, t["lse"], dqkv, B, T, H, prefix=W.prefix, causal=causal, rope=rope)
+        attention_backward(t, do, dqkv, B, T, H, W.prefix, causal, rope)
         lib.cast_colsum(dqkv, None, gw.qkv.b, M, 3 * D)
         dgrad(dqkv, bw.qkv.w, dh, M)
         wgrad(dqkv, t["h1"], gw.qkv.w, M)
@@ -248,7 +260,7 @@ def _tower_blocks_backward_drop(W: TowerW, G: TowerW, tape: list, g: torch.Tenso
         dgrad(gb, bw.proj.w, do, M1)
         wgrad(gb, t["o"], gw.proj.w, M1)
         dqkv = _e((M1, 3 * D), BF, dev)
-        lib.attention_bwd(t["qkv"], t["o"], do, t["lse"], dqkv, n1, T, H, prefix=W.prefix, rope=rope)
+        attention_backward(t, do, dqkv, n1, T, H, W.prefix, False, rope)
         lib.cast_colsum(dqkv, None, gw.qkv.b, M1, 3 * D)
         dh = _e((M1, D), BF, dev)
         dgrad(dqkv, bw.qkv.w, dh, M1)
