@@ -274,6 +274,26 @@ int vtp_latent_stats(const void* lat, int dtype, int B, int C, int HW, double* s
 int vtp_crop_resize_norm(const uint8_t* src_nhwc, int B, int H, int W, const int* src_idx, const float* boxes_xywh,
                          const uint8_t* flips, float* out_nchw, int N, int S, const float* mean3, const float* std3,
                          vtp_stream_t stream);
+/* The same crops with DINOv2's photometric augmentations between the resample and the normalisation, per crop n:
+ *   v / 255 in [0, 1] -> colour jitter (4 ops in the crop's order) -> grayscale -> Gaussian blur -> solarise
+ *   -> (x - mean[c]) / std[c]
+ * following torchvision.transforms.v2.functional on float images: brightness / contrast / saturation are _blend with a
+ * clamp to [0, 1] after each; contrast blends towards the scalar mean of rgb_to_grayscale over the whole crop as it stands
+ * when contrast runs; grayscale = 0.2989 r + 0.587 g + 0.114 b; hue through _rgb_to_hsv / _hsv_to_rgb, the shifted hue
+ * wrapped by a floored remainder(1); blur = 9 taps, weights exp(-x^2 / 2 sigma^2) normalised over x = -4..4, reflect
+ * padding at the crop border (hence S >= 5); solarise = x >= t ? 1 - x : x.
+ * params: fp32 [N][8], 16-byte aligned (device), one row per crop:
+ *   [0..3] brightness, contrast, saturation factors, hue shift (read only when [4] >= 0)
+ *   [4]    jitter order: index 0..23 into itertools.permutations(range(4)) (0 brightness, 1 contrast, 2 saturation,
+ *          3 hue), or -1 = no jitter
+ *   [5]    grayscale (3 equal channels) if != 0
+ *   [6]    blur sigma, 0 = no blur
+ *   [7]    solarise threshold t, 2.0 = off
+ * A row with every stage off gives the bit-identical output of vtp_crop_resize_norm.  mean_ws: fp32 [N] device workspace
+ * (the contrast means).  No atomics: repeat launches are bit-identical. */
+int vtp_crop_augment(const uint8_t* src_nhwc, int B, int H, int W, const int* src_idx, const float* boxes_xywh,
+                     const uint8_t* flips, const float* params, float* mean_ws, float* out_nchw, int N, int S,
+                     const float* mean3, const float* std3, vtp_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -8,13 +8,22 @@ crop on the device; masks are drawn on the device; caption tokenisation (pure-Py
 `vtp/tokenizers/text_tokenizer.py:208-257`) runs in a worker thread under the previous step.
 
 Crop geometry = torchvision `RandomResizedCrop.get_params` (area scale x log-uniform aspect ratio, 10 tries, centre-crop
-fallback) with DINOv2's scales (global 0.32-1, local 0.05-0.32) and OpenCLIP's (0.9-1) for the contrastive view; photometric
-augmentations (colour jitter, blur, solarise) are NOT implemented.  Masks: exactly round(mask_ratio * HW) patches on exactly
-round(mask_prob * 2B) global crops (SURVEY.md §8d), static shapes so that the step stays CUDA-graph replayable."""
+fallback) with DINOv2's scales (global 0.32-1, local 0.05-0.32) and OpenCLIP's (0.9-1) for the contrastive view.
+
+Photometric augmentations (`TrainBatchPipeline(photometric=PhotometricAug())`, off by default) follow DINOv2's multi-crop
+recipe on the self-distillation crops only: colour jitter (p 0.8; brightness / contrast 0.4, saturation 0.2, hue 0.1, random
+order), grayscale (p 0.2), Gaussian blur (9 taps, sigma U[0.1, 2]; p 1.0 / 0.1 / 0.5 on global view 1 / global view 2 /
+local crops), solarise (p 0.2, global view 2 only).  The host draws one 8-float row per crop (`photometric_params`) and
+`csrc/data.cu` applies them in the same pass that cuts the crop, with torchvision.transforms.v2.functional's float-image
+semantics.  Deliberate differences from DINOv2's PIL pipeline: the resample is bilinear (DINOv2: bicubic) and every stage
+stays fp32 (PIL rounds to uint8 after each op).  The CLIP and reconstruction views are never augmented.
+
+Masks: exactly round(mask_ratio * HW) patches on exactly round(mask_prob * 2B) global crops (SURVEY.md §8d), static shapes so that the step stays CUDA-graph replayable."""
 from __future__ import annotations
 
 import math
 from concurrent.futures import Future, ThreadPoolExecutor
+from dataclasses import dataclass
 from typing import Callable, Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -55,6 +64,42 @@ def random_resized_crop_boxes(rng: np.random.Generator, n: int, H: int, W: int, 
     return out
 
 
+@dataclass(frozen=True)
+class PhotometricAug:
+    """DINO / DINOv2 photometric recipe for the self-distillation crops (defaults = the published values)."""
+    jitter_p: float = 0.8
+    brightness: float = 0.4          # factor U[1 - b, 1 + b]
+    contrast: float = 0.4            # factor U[1 - c, 1 + c]
+    saturation: float = 0.2          # factor U[1 - s, 1 + s]
+    hue: float = 0.1                 # shift U[-h, h]
+    gray_p: float = 0.2
+    blur_sigma: Tuple[float, float] = (0.1, 2.0)
+    blur_p: Tuple[float, float, float] = (1.0, 0.1, 0.5)   # global view 1, global view 2, local crops
+    solarize_p: float = 0.2          # global view 2 only
+    solarize_threshold: float = 128 / 255
+
+
+PHOTO_OFF = (0.0, 0.0, 0.0, 0.0, -1.0, 0.0, 0.0, 2.0)   # a params row with every stage off
+
+
+def photometric_params(rng: np.random.Generator, n: int, aug: PhotometricAug, blur_p: float, solarize_p: float) -> np.ndarray:
+    """n rows of the vtp_crop_augment table (fp32 [n, 8], layout in include/vtp_b200.h): jitter factors and a uniform
+    order code 0..23 into itertools.permutations(range(4)) (-1 = no jitter), grayscale flag, blur sigma (0 = off),
+    solarise threshold (2.0 = off)."""
+    out = np.empty((n, 8), dtype=np.float32)
+    jit = rng.random(n) < aug.jitter_p
+    out[:, 0] = rng.uniform(1 - aug.brightness, 1 + aug.brightness, n)
+    out[:, 1] = rng.uniform(1 - aug.contrast, 1 + aug.contrast, n)
+    out[:, 2] = rng.uniform(1 - aug.saturation, 1 + aug.saturation, n)
+    out[:, 3] = rng.uniform(-aug.hue, aug.hue, n)
+    out[:, 4] = np.where(jit, rng.integers(0, 24, n), -1)
+    out[:, 5] = rng.random(n) < aug.gray_p
+    sigma = rng.uniform(aug.blur_sigma[0], aug.blur_sigma[1], n)
+    out[:, 6] = np.where(rng.random(n) < blur_p, sigma, 0.0)
+    out[:, 7] = np.where(rng.random(n) < solarize_p, aug.solarize_threshold, 2.0)
+    return out
+
+
 def ibot_masks(n_images: int, HW: int, mask_ratio: float, mask_prob: float, device, generator: Optional[torch.Generator] = None):
     """Device-side iBOT masks of fixed size: (mask_indices int64 ascending flat indices into [n_images*HW],
     masks_weight fp32 = 1 / #masked patches of that image) — `mask_indices_list` / `masks_weight` of vtp.py:434,472."""
@@ -80,7 +125,8 @@ class TrainBatchPipeline:
     def __init__(self, device="cuda", *, image_size: int = 256, local_size: int = 96, n_local: int = 8, patch: int = 16,
                  global_scale=(0.32, 1.0), local_scale=(0.05, 0.32), clip_scale=(0.9, 1.0), mask_ratio: float = 0.3,
                  mask_prob: float = 0.5, tokenizer: Optional[Callable[[Sequence[str]], torch.Tensor]] = None, seed: int = 0,
-                 clip_norm=(CLIP_MEAN, CLIP_STD), image_norm=(IMAGENET_MEAN, IMAGENET_STD)):
+                 clip_norm=(CLIP_MEAN, CLIP_STD), image_norm=(IMAGENET_MEAN, IMAGENET_STD),
+                 photometric: Optional[PhotometricAug] = None):
         self.device = torch.device(device)
         self.S, self.Sl, self.n_local, self.patch = image_size, local_size, n_local, patch
         self.scales = dict(g=global_scale, l=local_scale, c=clip_scale)
@@ -90,12 +136,19 @@ class TrainBatchPipeline:
         self.gen = torch.Generator(device=self.device)
         self.gen.manual_seed(seed)
         self.clip_norm, self.image_norm = clip_norm, image_norm
+        # photometric rows come from their own generator, so boxes, flips and masks do not depend on `photometric`;
+        # per step: global view 1 (B rows), global view 2 (B rows), local crops (n_local * B rows), in that order
+        self.photometric = photometric
+        self.photo_rng = np.random.default_rng([seed, 1])
+        self._mean_ws: Dict[int, torch.Tensor] = {}
         self.stream = torch.cuda.Stream(self.device)
         self.pool = ThreadPoolExecutor(max_workers=1)
         self._queue: List[Tuple[Dict[str, torch.Tensor], torch.cuda.Event, Optional[Future]]] = []
 
-    def _crops(self, src: torch.Tensor, n_per: int, size: int, scale, norm, flip: bool = True) -> torch.Tensor:
-        """n_per crops per source image, crop-major [n_per * B] (crop j of image b at row j * B + b)."""
+    def _crops(self, src: torch.Tensor, n_per: int, size: int, scale, norm, flip: bool = True,
+               photo: Optional[np.ndarray] = None) -> torch.Tensor:
+        """n_per crops per source image, crop-major [n_per * B] (crop j of image b at row j * B + b); `photo`: one
+        vtp_crop_augment row per crop, or None for plain crops."""
         B, H, W, _ = src.shape
         N = n_per * B
         boxes = random_resized_crop_boxes(self.rng, N, H, W, scale)
@@ -106,7 +159,13 @@ class TrainBatchPipeline:
         ix = torch.from_numpy(idx).pin_memory().to(dev, non_blocking=True)
         fl = torch.from_numpy(flips).pin_memory().to(dev, non_blocking=True)
         out = torch.empty((N, 3, size, size), dtype=torch.float32, device=dev)
-        lib.crop_resize_norm(src, ix, bx, fl, out, mean=norm[0], std=norm[1])
+        if photo is None:
+            lib.crop_resize_norm(src, ix, bx, fl, out, mean=norm[0], std=norm[1])
+            return out
+        prm = torch.from_numpy(photo).pin_memory().to(dev, non_blocking=True)
+        if N not in self._mean_ws:
+            self._mean_ws[N] = torch.empty(N, dtype=torch.float32, device=dev)
+        lib.crop_augment(src, ix, bx, fl, prm, self._mean_ws[N], out, mean=norm[0], std=norm[1])
         return out
 
     def submit(self, images_u8: torch.Tensor, captions=None) -> None:
@@ -126,10 +185,16 @@ class TrainBatchPipeline:
             src = images_u8.to(self.device, non_blocking=True).contiguous()
             B = src.shape[0]
             HW = (self.S // self.patch) ** 2
+            pg = pl = None
+            if self.photometric is not None:
+                a, r = self.photometric, self.photo_rng
+                pg = np.concatenate([photometric_params(r, B, a, a.blur_p[0], 0.0),
+                                     photometric_params(r, B, a, a.blur_p[1], a.solarize_p)])
+                pl = photometric_params(r, self.n_local * B, a, a.blur_p[2], 0.0)
             batch = dict(
                 image=self._crops(src, 1, self.S, self.scales["c"], self.clip_norm, flip=False),
-                global_crops=self._crops(src, 2, self.S, self.scales["g"], self.image_norm),      # view-major [2B]
-                local_crops=self._crops(src, self.n_local, self.Sl, self.scales["l"], self.image_norm),
+                global_crops=self._crops(src, 2, self.S, self.scales["g"], self.image_norm, photo=pg),  # view-major [2B]
+                local_crops=self._crops(src, self.n_local, self.Sl, self.scales["l"], self.image_norm, photo=pl),
                 rec_image=self._crops(src, 1, self.S, (1.0, 1.0), self.image_norm, flip=False),
             )
             batch["mask_indices"], batch["masks_weight"] = ibot_masks(2 * B, HW, self.mask_ratio, self.mask_prob, self.device, self.gen)

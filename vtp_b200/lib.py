@@ -120,6 +120,9 @@ SIGNATURES: dict[str, tuple] = {
     "vtp_comm_close_handle": (C.c_int, [C.c_void_p]),
     "vtp_crop_resize_norm": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.c_int, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_void_p]),
+    "vtp_crop_augment": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                   C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_float),
+                                   C.c_void_p]),
     "vtp_comm_barrier": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_long, C.c_void_p, C.c_void_p, C.c_void_p]),
 }
 
@@ -501,3 +504,31 @@ def crop_resize_norm(src_u8, src_idx, boxes, flips, out, mean=(0.485, 0.456, 0.4
     sd = (C.c_float * 3)(*std)
     check(load().vtp_crop_resize_norm(_ptr(src_u8), B, H, W, _ptr(src_idx), _ptr(boxes), _ptr(flips), _ptr(out), N, S, m, sd,
                                       _st(stream)), "vtp_crop_resize_norm")
+
+
+def crop_augment(src_u8, src_idx, boxes, flips, params, mean_ws, out, mean=(0.485, 0.456, 0.406), std=(0.229, 0.224, 0.225),
+                 stream=None):
+    """crop_resize_norm with DINOv2's photometric augmentations between the resample and the normalisation.
+    params fp32 [N,8] (16-byte aligned; layout in include/vtp_b200.h), mean_ws fp32 [N] workspace; out fp32 [N,3,S,S]
+    with S >= 5; the rest as in crop_resize_norm."""
+    import torch
+
+    B, H, W, _ = src_u8.shape
+    N, _, S, _ = out.shape
+    if src_u8.dtype != torch.uint8 or src_u8.shape[-1] != 3 or not src_u8.is_contiguous():
+        raise VtpError(f"crop_augment: src must be contiguous uint8 [B,H,W,3], got {src_u8.dtype} {tuple(src_u8.shape)}")
+    if out.dtype != torch.float32 or tuple(out.shape) != (N, 3, S, S) or not out.is_contiguous():
+        raise VtpError(f"crop_augment: out must be contiguous fp32 [N,3,S,S], got {out.dtype} {tuple(out.shape)}")
+    for name, t, dt, shape in (("src_idx", src_idx, torch.int32, (N,)), ("boxes", boxes, torch.float32, (N, 4)),
+                               ("params", params, torch.float32, (N, 8)), ("mean_ws", mean_ws, torch.float32, (N,)),
+                               ("flips", flips, torch.uint8, (N,))):
+        if t is None and name == "flips":
+            continue
+        if t.dtype != dt or tuple(t.shape) != shape or not t.is_contiguous():
+            raise VtpError(f"crop_augment: {name} must be contiguous {dt} {list(shape)}, got {t.dtype} {tuple(t.shape)}")
+    if params.data_ptr() % 16:
+        raise VtpError("crop_augment: params must be 16-byte aligned")
+    m = (C.c_float * 3)(*mean)
+    sd = (C.c_float * 3)(*std)
+    check(load().vtp_crop_augment(_ptr(src_u8), B, H, W, _ptr(src_idx), _ptr(boxes), _ptr(flips), _ptr(params), _ptr(mean_ws),
+                                  _ptr(out), N, S, m, sd, _st(stream)), "vtp_crop_augment")
