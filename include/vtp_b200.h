@@ -139,7 +139,8 @@ int vtp_attention_fwd_f32(const float* qkv, float* out, int B, int T, int H, int
  * forward stages above plus restated losses and a fused optimiser)
  * ------------------------------------------------------------------------------------------------------------ */
 /* dual of vtp_attention_fwd incl. the RoPE rotation (layers/attention.py:70-89,110-126): dqkv = d/d(pre-RoPE qkv).
- * Single pass, the whole sequence in one CTA: HW = T - prefix <= 256 (VTP_ERR_ARG above; see vtp_attention_bwd_long) */
+ * Single pass, HW = T - prefix <= 256 (VTP_ERR_ARG above; see vtp_attention_bwd_long): one CTA per sequence, or a
+ * cluster of two CTAs for non-causal 128 < HW <= 256.  No workspace; repeat launches are bit-identical. */
 int vtp_attention_bwd(const void* qkv, const void* o, const void* dout, const float* lse, void* dqkv,
                       const void* rope_sin, const void* rope_cos, int B, int T, int H, int prefix, int causal,
                       vtp_stream_t stream);

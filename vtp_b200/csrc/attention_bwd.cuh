@@ -4,6 +4,8 @@
 
 namespace vtp {
 
+constexpr float LOG2E = 1.4426950408889634f;
+
 __device__ __forceinline__ float ex2f(float x) {  // ex2.approx.ftz: no denormal slow path (exp2f() costs 4 extra instr)
     float y;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -67,6 +69,39 @@ __device__ __forceinline__ void rope_bwd_frag(float (&g)[16], const __nv_bfloat1
             g[2 * (jn + 4) + c] = b * ch[c] - a * sl[c];
         }
     }
+}
+
+// m64n64 accumulator fragment (element 4 jn + 2 i + c: row i of this thread, column 8 jn + 2 c4 + c) -> bf16 register A
+// operands of the 4 k-steps of 16 columns (wgmma_m64n64_rs): a[kk][q] holds columns 16 kk + 8 (q >> 1) + 2 c4 + {0, 1}
+// of row q & 1.  Callers select P and dS to 0 outside the valid rows and columns before packing: there lse and δ may be
+// anything, so multiplying by 0 could give NaN.
+__device__ __forceinline__ void pack_a(const float (&x)[32], uint32_t (&a)[4][4]) {
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+        a[kk][0] = pack_bf16x2(x[8 * kk], x[8 * kk + 1]), a[kk][1] = pack_bf16x2(x[8 * kk + 2], x[8 * kk + 3]);
+        a[kk][2] = pack_bf16x2(x[8 * kk + 4], x[8 * kk + 5]), a[kk][3] = pack_bf16x2(x[8 * kk + 6], x[8 * kk + 7]);
+    }
+}
+
+// Row i of an m64n64 fragment of 64-dim gradients (one token row, dims 8 jn + 2 c4 + c in this thread) to bf16 at drow:
+// plus w · cls (the rank-1 term of the cls token, when cls is given), then RoPEᵀ (when sin_row is given)
+__device__ __forceinline__ void store_grad_row(const float (&acc)[32], int i, float w, const __nv_bfloat16* cls,
+                                               const __nv_bfloat16* sin_row, const __nv_bfloat16* cos_row,
+                                               __nv_bfloat16* drow, int c4) {
+    float g[16];
+#pragma unroll
+    for (int e = 0; e < 16; ++e) g[e] = acc[4 * (e >> 1) + 2 * i + (e & 1)];
+    if (cls) {
+#pragma unroll
+        for (int jn = 0; jn < 8; ++jn) {
+            const uint32_t x = __ldg(reinterpret_cast<const uint32_t*>(cls + 8 * jn + 2 * c4));
+            g[2 * jn] += w * bf16_lo(x), g[2 * jn + 1] += w * bf16_hi(x);
+        }
+    }
+    if (sin_row) rope_bwd_frag(g, sin_row, cos_row, c4);
+#pragma unroll
+    for (int jn = 0; jn < 8; ++jn)
+        *reinterpret_cast<uint32_t*>(drow + 8 * jn + 2 * c4) = pack_bf16x2(g[2 * jn], g[2 * jn + 1]);
 }
 
 }  // namespace vtp

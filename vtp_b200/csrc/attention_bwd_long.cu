@@ -38,7 +38,6 @@ constexpr int DQ_SMEM = DQ_BAR + 128 + 1024;  // + alignment slack
 constexpr int KV_K = 0, KV_V = BL_TILE, KV_QD = 2 * BL_TILE, KV_LD = KV_QD + BL_NSTAGE * 2 * BL_TILE;
 constexpr int KV_BAR = KV_LD + BL_NSTAGE * 1024;
 constexpr int KV_SMEM = KV_BAR + 128 + 1024;
-constexpr float LOG2E = 1.4426950408889634f;
 
 struct AttnBwdLongDev {
     const __nv_bfloat16* qkv;   // [B*T][3D] post-RoPE q,k ; v
@@ -77,17 +76,6 @@ __global__ void __launch_bounds__(256) attn_bwd_delta_kernel(const AttnBwdLongDe
         const int h = (int)(pair - tok * p.H);
         const long b = tok / p.T;
         p.delta[(b * p.H + h) * p.T + (tok - b * p.T)] = acc;
-    }
-}
-
-// m64n64 accumulator fragment (element 4 jn + 2 i + c: row i of this thread, column 8 jn + 2 c4 + c) -> bf16 register A
-// operands of the 4 k-steps of 16 columns (wgmma_m64n64_rs).  Callers select P and dS to 0 outside the valid rows and
-// columns before packing: there lse and δ may be anything, so multiplying by 0 could give NaN.
-__device__ __forceinline__ void pack_a(const float (&x)[32], uint32_t (&a)[4][4]) {
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-        a[kk][0] = pack_bf16x2(x[8 * kk], x[8 * kk + 1]), a[kk][1] = pack_bf16x2(x[8 * kk + 2], x[8 * kk + 3]);
-        a[kk][2] = pack_bf16x2(x[8 * kk + 4], x[8 * kk + 5]), a[kk][3] = pack_bf16x2(x[8 * kk + 6], x[8 * kk + 7]);
     }
 }
 
@@ -196,25 +184,14 @@ __global__ void __launch_bounds__(BL_THREADS, 1) attn_bwd_long_dq_kernel(const _
             __syncwarp();
             if (lane == 0) mbar_arrive(empty + st);
         }
-        // epilogue: dq[4 jn + 2 i + c] is dim 8 jn + 2 c4 + c of row i; rows >= HW are not stored
+        // epilogue: rows >= HW are not stored
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
             if (!qvalid[i]) continue;
-            float gq[16];
-#pragma unroll
-            for (int e = 0; e < 16; ++e) gq[e] = dq[4 * (e >> 1) + 2 * i + (e & 1)];
-            if (prefix > 0) {
-#pragma unroll
-                for (int jn = 0; jn < 8; ++jn) {
-                    const uint32_t w = __ldg(reinterpret_cast<const uint32_t*>(kcls + 8 * jn + 2 * c4));
-                    gq[2 * jn] += ds_cls[i] * bf16_lo(w), gq[2 * jn + 1] += ds_cls[i] * bf16_hi(w);
-                }
-            }
-            if (p.rope_sin) rope_bwd_frag(gq, p.rope_sin + (long)qi[i] * 64, p.rope_cos + (long)qi[i] * 64, c4);
-            __nv_bfloat16* drow = p.dqkv + (row0 + prefix + qi[i]) * 3 * D + h * 64;
-#pragma unroll
-            for (int jn = 0; jn < 8; ++jn)
-                *reinterpret_cast<uint32_t*>(drow + 8 * jn + 2 * c4) = pack_bf16x2(gq[2 * jn], gq[2 * jn + 1]);
+            const bool rope = p.rope_sin != nullptr;
+            store_grad_row(dq, i, ds_cls[i], prefix > 0 ? kcls : nullptr, rope ? p.rope_sin + (long)qi[i] * 64 : nullptr,
+                           rope ? p.rope_cos + (long)qi[i] * 64 : nullptr,
+                           p.dqkv + (row0 + prefix + qi[i]) * 3 * D + h * 64, c4);
         }
     } else {
         setmaxnreg_dec<104>();
@@ -350,32 +327,15 @@ __global__ void __launch_bounds__(BL_THREADS, 1) attn_bwd_long_dkdv_kernel(const
             __syncwarp();
             if (lane == 0) mbar_arrive(empty + st);
         }
-        // epilogue: my key rows kj; acc[4 jn + 2 i + c] = dim 8 jn + 2 c4 + c; rows >= HW are not stored
+        // epilogue: my key rows kj; rows >= HW are not stored
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
             if (!kvalid[i]) continue;
-            float gv[16], gk[16];
-#pragma unroll
-            for (int e = 0; e < 16; ++e) {
-                const int jn = e >> 1, cc = e & 1;
-                gv[e] = dv[4 * jn + 2 * i + cc], gk[e] = dk[4 * jn + 2 * i + cc];
-            }
-            if (prefix > 0) {
-#pragma unroll
-                for (int jn = 0; jn < 8; ++jn) {
-                    const uint32_t wd = __ldg(reinterpret_cast<const uint32_t*>(docls + 8 * jn + 2 * c4));
-                    const uint32_t wq = __ldg(reinterpret_cast<const uint32_t*>(qcls + 8 * jn + 2 * c4));
-                    gv[2 * jn] += p0j[i] * bf16_lo(wd), gv[2 * jn + 1] += p0j[i] * bf16_hi(wd);
-                    gk[2 * jn] += ds0j[i] * bf16_lo(wq), gk[2 * jn + 1] += ds0j[i] * bf16_hi(wq);
-                }
-            }
-            if (p.rope_sin) rope_bwd_frag(gk, p.rope_sin + (long)kj[i] * 64, p.rope_cos + (long)kj[i] * 64, c4);
+            const bool rope = p.rope_sin != nullptr;
             __nv_bfloat16* drow = p.dqkv + (row0 + prefix + kj[i]) * 3 * D + h * 64;
-#pragma unroll
-            for (int jn = 0; jn < 8; ++jn) {
-                *reinterpret_cast<uint32_t*>(drow + 2 * D + 8 * jn + 2 * c4) = pack_bf16x2(gv[2 * jn], gv[2 * jn + 1]);
-                *reinterpret_cast<uint32_t*>(drow + D + 8 * jn + 2 * c4) = pack_bf16x2(gk[2 * jn], gk[2 * jn + 1]);
-            }
+            store_grad_row(dv, i, p0j[i], prefix > 0 ? docls : nullptr, nullptr, nullptr, drow + 2 * D, c4);
+            store_grad_row(dk, i, ds0j[i], prefix > 0 ? qcls : nullptr, rope ? p.rope_sin + (long)kj[i] * 64 : nullptr,
+                           rope ? p.rope_cos + (long)kj[i] * 64 : nullptr, drow + D, c4);
         }
     } else {
         setmaxnreg_dec<104>();

@@ -53,6 +53,31 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     }
 }
 
+// ---------------------------------------------------------------- thread-block clusters (distributed shared memory)
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return r;
+}
+// every thread of every CTA of the cluster: shared-memory writes before it are visible to cluster-scope reads after it
+__device__ __forceinline__ void cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// the address of the same shared-memory location in CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t mapa_shared(uint32_t saddr, uint32_t rank) {
+    uint32_t r;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(rank));
+    return r;
+}
+__device__ __forceinline__ float4 ld_shared_cluster_f4(uint32_t caddr) {
+    float4 v;
+    asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];"
+                 : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
+                 : "r"(caddr)
+                 : "memory");
+    return v;
+}
+
 // ---------------------------------------------------------------- fences
 __device__ __forceinline__ void fence_proxy_async_smem() {
     // generic-proxy smem writes -> visible to the async proxy (wgmma / TMA reads)
