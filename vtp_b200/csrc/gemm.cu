@@ -985,9 +985,9 @@ extern "C" int vtp_gemm_bf16(const vtp_gemm_args* a, vtp_stream_t stream_) {
             uint32_t box[2] = {64, 32};
             int rc = make_tmap(&tmP, a->out2, VTP_BF16, 2, dims, strides, box);
             if (rc) return rc;
-            return launch_gemm<128, 2, VTP_ACT_SWIGLU8, false, 6>(tmA, tmB, p, stream, &tmH, &tmP);
+            return launch_gemm<128, 4, VTP_ACT_SWIGLU8, false, 6>(tmA, tmB, p, stream, &tmH, &tmP);
         }
-        return launch_gemm<128, 3, VTP_ACT_SWIGLU8, false, 7>(tmA, tmB, p, stream, &tmH);
+        return launch_gemm<128, 4, VTP_ACT_SWIGLU8, false, 7>(tmA, tmB, p, stream, &tmH);
     }
     if (fast) {
         CUtensorMap tmO;
@@ -1007,7 +1007,7 @@ extern "C" int vtp_gemm_bf16(const vtp_gemm_args* a, vtp_stream_t stream_) {
         const int mode = a->mask_pos ? 5 : (a->out_dtype == VTP_F32 ? 3 : 1) + (a->resid ? 1 : 0);
 #define VTP_FAST_CFG(ACT_, MODE_)                                                                                     \
     return BN == 64 ? launch_gemm<64, 4, ACT_, false, MODE_>(tmA, tmB, p, stream, &tmO)                              \
-                    : launch_gemm<128, 3, ACT_, false, MODE_>(tmA, tmB, p, stream, &tmO)
+                    : launch_gemm<128, 4, ACT_, false, MODE_>(tmA, tmB, p, stream, &tmO)
         if (mode == 5) VTP_FAST_CFG(VTP_ACT_NONE, 5);  // LPIPS dgrad with the ReLU mask: bf16 out, no bias / activation
 #define VTP_FAST_ACT(ACT_)                                 \
     do {                                                   \
@@ -1025,7 +1025,7 @@ extern "C" int vtp_gemm_bf16(const vtp_gemm_args* a, vtp_stream_t stream_) {
     }
 #define VTP_LAUNCH(ACT_, PS_)                                                              \
     return BN == 64 ? launch_gemm<64, 4, ACT_, PS_>(tmA, tmB, p, stream)                  \
-                    : launch_gemm<128, 3, ACT_, PS_>(tmA, tmB, p, stream)
+                    : launch_gemm<128, 4, ACT_, PS_>(tmA, tmB, p, stream)
     if (a->ps_r > 0) {
         VTP_CHECK_ARG(a->act == VTP_ACT_NONE, "gemm: pixel shuffle has no activation");
         VTP_LAUNCH(VTP_ACT_NONE, true);
@@ -1033,7 +1033,7 @@ extern "C" int vtp_gemm_bf16(const vtp_gemm_args* a, vtp_stream_t stream_) {
     switch (a->act) {
         case VTP_ACT_NONE: VTP_LAUNCH(VTP_ACT_NONE, false);
         case VTP_ACT_GELU: VTP_LAUNCH(VTP_ACT_GELU, false);
-        case VTP_ACT_SWIGLU8: return launch_gemm<128, 3, VTP_ACT_SWIGLU8, false>(tmA, tmB, p, stream);
+        case VTP_ACT_SWIGLU8: return launch_gemm<128, 4, VTP_ACT_SWIGLU8, false>(tmA, tmB, p, stream);
         case VTP_ACT_ROPE: VTP_LAUNCH(VTP_ACT_ROPE, false);
         case VTP_ACT_RELU: VTP_LAUNCH(VTP_ACT_RELU, false);
         default: VTP_FAIL(VTP_ERR_ARG, "gemm: unknown activation %d", a->act);
