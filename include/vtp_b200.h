@@ -296,6 +296,43 @@ int vtp_crop_augment(const uint8_t* src_nhwc, int B, int H, int W, const int* sr
                      const uint8_t* flips, const float* params, float* mean_ws, float* out_nchw, int N, int S,
                      const float* mean3, const float* std3, vtp_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Linear probing on frozen trunk features (vtp_b200/csrc/probe.cu): the grid of fp32 linear classifiers of
+ * tools/test_linear_probing_hf.py, trained with SGD-momentum and a cosine schedule.  G classifiers of C classes each,
+ * padded to Cp = C rounded up to 8 columns; their logits sit side by side in Z [B][ldz] (classifier g owns columns
+ * [g*Cp, g*Cp + C)).  The classifier GEMMs (forward, dW) are vtp_gemm_bf16 on bf16x3 operands (vtp_split3).
+ * ------------------------------------------------------------------------------------------------------------ */
+/* tools/test_linear_probing_hf.py:119-152 (get_intermediate_layers_feature + create_linear_input) read in place from
+ * the fp32 residual stream x [B*T][D] (row 0 of every image is the cls token) after one of the last blocks:
+ *   X[b][cls_col + :D]  = final_norm(x[b*T])                               (the block's cls token)
+ *   X[b][mean_col + :D] = (Σ_{t=1..T-1} final_norm(x[b*T+t])) / (T-1)      if mean_col >= 0 (patch mean, t ascending)
+ * final_norm = RMSNorm (b == NULL) or LayerNorm with the arithmetic of vtp_norm_fwd (fp32 out).  X fp32 [B][ldX].
+ * One CTA per image, no atomics. */
+int vtp_probe_features(const float* x, int B, int T, int D, const float* w, const float* b, float eps, float* X, long ldX,
+                       int cls_col, int mean_col, vtp_stream_t stream);
+/* tools/test_linear_probing_hf.py:285-286 (nn.CrossEntropyLoss, mean over the batch, per classifier) on fp32 logits Z
+ * [B][ldz] with int64 labels [B] in [0, C): loss_acc[g] += mean_b (lse_b - Z[b][g*Cp + label_b]) (NaN for a label out
+ * of range), and dZ = (softmax - onehot) / B written as the bf16x3 wgrad operand, rows stacked hi|hi|lo:
+ * dZ3[r][:] = hi(dZ[r]), dZ3[B+r][:] = hi(dZ[r]), dZ3[2B+r][:] = lo(dZ[r]) (bf16 [3B][ldd], padding columns 0), and
+ * dbias[g*Cp + c] = Σ_b dZ[b][g*Cp + c] summed in ascending b.  One CTA per classifier, no atomics. */
+int vtp_probe_ce(const float* Z, long ldz, int B, int G, int C, int Cp, const int64_t* labels, float* loss_acc,
+                 void* dZ3, long ldd, float* dbias, vtp_stream_t stream);
+/* tools/test_linear_probing_hf.py:487-488,291 (torch.optim.SGD(momentum, dampening 0, weight decay 0) stepped by
+ * CosineAnnealingLR) over one region of n fp32 parameters laid out as rows of row_len, rows_per_cls rows per
+ * classifier, classifier index cls0 + row / rows_per_cls:
+ *   g' = g * gscale;  buf = (step == 1) ? g' : buf * momentum + g';  p = p - lr * buf
+ * with step = hyper[0] (the device step counter advanced by vtp_hyper_tick) and lr = lr_table[(step-1) * lr_ld + cls]
+ * (the last row past n_steps rows).  pb (optional, bf16 [rows][3*row_len]) receives the refreshed hi|lo|hi B operand
+ * (vtp_split3 b_side = 1) of the new weights.  n, row_len (when pb is given) and rows_per_cls * row_len are multiples
+ * of 4.  The gradient is left as it is (every step overwrites it). */
+int vtp_probe_sgd(float* p, const float* g, float* buf, long n, int row_len, int rows_per_cls, int cls0,
+                  const float* lr_table, int lr_ld, int n_steps, const float* hyper, float momentum, float gscale,
+                  void* pb, vtp_stream_t stream);
+/* tools/test_linear_probing_hf.py:326-328: counts[g] += #{b : argmax_c Z[b][g*Cp + c] == labels[b]} with torch.argmax's
+ * rules (first maximal index; NaN counts as the maximum, the first NaN wins). */
+int vtp_probe_correct(const float* Z, long ldz, int B, int G, int C, int Cp, const int64_t* labels, int64_t* counts,
+                      vtp_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -12,7 +12,7 @@ Two precision modes, selected by the caller (VTPModel maps them from the autocas
 from __future__ import annotations
 
 from dataclasses import dataclass, field
-from typing import Dict, List, Optional, Sequence, Tuple
+from typing import Callable, Dict, List, Optional, Sequence, Tuple
 
 import torch
 
@@ -324,11 +324,12 @@ def _block_drop(W: TowerW, bw: BlockW, x: torch.Tensor, B: int, T: int, rope, dr
 
 def tower_blocks(W: TowerW, x: torch.Tensor, B: int, T: int, rope, mode: str, *, causal: bool = False,
                  tape: Optional[list] = None, taps: Optional[Dict[int, torch.Tensor]] = None,
-                 drop: Optional[DropPlan] = None) -> torch.Tensor:
+                 drop: Optional[DropPlan] = None, hook: Optional[Callable[[int, torch.Tensor], None]] = None) -> torch.Tensor:
     """The block loop (encoders/vision_transformer.py:228-233, decoders/pixel_decoder.py:147-148,
     encoders/text_transformer.py:100-104): x [B*T, D] residual stream (fp32, or bf16 for the autocast decoder).
     Inference updates x in place; with a tape every sub-layer writes a fresh stream buffer and saves what backward
-    needs.  `taps` {block index: None} is filled with copies of the stream after those blocks."""
+    needs.  `taps` {block index: None} is filled with copies of the stream after those blocks; `hook(li, x)` is called
+    after every block with the stream itself (read it before returning: inference overwrites it in place)."""
     dev = x.device
     M, D, H = B * T, W.D, W.heads
     act = BF if mode == "bf16" else F32
@@ -343,6 +344,8 @@ def tower_blocks(W: TowerW, x: torch.Tensor, B: int, T: int, rope, mode: str, *,
                 tape.append(t)
             if taps is not None and li in taps:
                 taps[li] = x.clone()
+            if hook is not None:
+                hook(li, x)
         return x
     for li, bw in enumerate(W.blocks):
         t = {} if tape is not None else None
@@ -393,6 +396,8 @@ def tower_blocks(W: TowerW, x: torch.Tensor, B: int, T: int, rope, mode: str, *,
         x = x_out
         if taps is not None and li in taps:
             taps[li] = x.clone()
+        if hook is not None:
+            hook(li, x)
     return x
 
 
@@ -422,14 +427,14 @@ def trunk_tokens(W: TowerW, img: torch.Tensor, mode: str, mask_idx: Optional[tor
 
 
 def trunk_forward(W: TowerW, img: torch.Tensor, mode: str, *, mask_idx=None, tape: Optional[dict] = None,
-                  taps=None, drop: Optional[DropPlan] = None):
+                  taps=None, drop: Optional[DropPlan] = None, hook=None):
     """encoders/vision_transformer.py:221-258 for one resolution group.  Returns (x_prenorm [B*T,D] fp32, meta)."""
     x, (B, T, gh, gw), a = trunk_tokens(W, img, mode, mask_idx)
     if tape is not None:
         tape["patch_a"] = a
     rope = W.rope(gh, gw, img.device)
     blk_tape = [] if tape is not None else None
-    x = tower_blocks(W, x, B, T, rope, mode, tape=blk_tape, taps=taps, drop=drop)
+    x = tower_blocks(W, x, B, T, rope, mode, tape=blk_tape, taps=taps, drop=drop, hook=hook)
     if tape is not None:
         tape["blocks"] = blk_tape
         tape["meta"] = (B, T, gh, gw)

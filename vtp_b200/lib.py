@@ -124,6 +124,14 @@ SIGNATURES: dict[str, tuple] = {
                                    C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_float),
                                    C.c_void_p]),
     "vtp_comm_barrier": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_long, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vtp_probe_features": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p,
+                                     C.c_long, C.c_int, C.c_int, C.c_void_p]),
+    "vtp_probe_ce": (C.c_int, [C.c_void_p, C.c_long, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                               C.c_long, C.c_void_p, C.c_void_p]),
+    "vtp_probe_sgd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_long, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
+                                C.c_int, C.c_void_p, C.c_float, C.c_float, C.c_void_p, C.c_void_p]),
+    "vtp_probe_correct": (C.c_int, [C.c_void_p, C.c_long, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                    C.c_void_p]),
 }
 
 
@@ -477,6 +485,32 @@ def comm_close_handle(ptr: int) -> None:
 def comm_barrier(pad_ptrs, rank: int, epoch: int, err_flag, poison=None, stream=None):
     check(load().vtp_comm_barrier(_ptr_array(pad_ptrs), len(pad_ptrs), rank, epoch, _ptr(err_flag), _ptr(poison), _st(stream)),
           "vtp_comm_barrier")
+
+
+# ------------------------------------------------------------------------------------------------ linear probing
+def probe_features(x, B: int, T: int, D: int, w, b, eps: float, X, *, cls_col: int, mean_col: int = -1, stream=None):
+    """X[:, cls_col:+D] = final_norm(cls row of x); X[:, mean_col:+D] = mean of the normalised patch rows (mean_col >= 0).
+    x fp32 [B*T, D] (the residual stream, read in place); X fp32 [B, ldX]."""
+    check(load().vtp_probe_features(_ptr(x), B, T, D, _ptr(w), _ptr(b), eps, _ptr(X), X.stride(0), cls_col, mean_col,
+                                    _st(stream)), "vtp_probe_features")
+
+
+def probe_ce(Z, B: int, G: int, Cn: int, Cp: int, labels, loss_acc, dZ3, dbias, stream=None):
+    check(load().vtp_probe_ce(_ptr(Z), Z.stride(0), B, G, Cn, Cp, _ptr(labels), _ptr(loss_acc), _ptr(dZ3), dZ3.stride(0),
+                              _ptr(dbias), _st(stream)), "vtp_probe_ce")
+
+
+def probe_sgd(p, g, buf, n: int, *, row_len: int, rows_per_cls: int, cls0: int, lr_table, hyper, momentum: float,
+              grad_scale: float = 1.0, pb=None, stream=None):
+    """lr_table fp32 [n_steps, G] (device); hyper: the step state advanced by hyper_tick."""
+    check(load().vtp_probe_sgd(_ptr(p), _ptr(g), _ptr(buf), n, row_len, rows_per_cls, cls0, _ptr(lr_table),
+                               lr_table.shape[1], lr_table.shape[0], _ptr(hyper), momentum, grad_scale, _ptr(pb),
+                               _st(stream)), "vtp_probe_sgd")
+
+
+def probe_correct(Z, B: int, G: int, Cn: int, Cp: int, labels, counts, stream=None):
+    check(load().vtp_probe_correct(_ptr(Z), Z.stride(0), B, G, Cn, Cp, _ptr(labels), _ptr(counts), _st(stream)),
+          "vtp_probe_correct")
 
 
 # ------------------------------------------------------------------------------------------------ image / latent formats
