@@ -219,6 +219,18 @@ int vtp_lpips_tap(const void* f0, const void* f1, const float* w, void* g0, long
                   vtp_stream_t stream);
 /* col2im of the conv1_1 input gradient + ScalingLayer backward: bf16 [B*H*W][32] -> fp32 NCHW d(image) */
 int vtp_lpips_img_grad(const void* dcol, float* dimg, int B, int H, int W, vtp_stream_t stream);
+/* fp32-accurate metric forward (tools/test_reconstruction_hf.py:379-388 runs the VGG in fp32): activations fp32 NHWC,
+ * conv operands bf16x3 ([hi|hi|lo] activations against [hi|lo|hi] weights, vtp_split3), conv GEMMs with fp32 out.
+ * prep3: 3x3 im2col of an fp32 NCHW image already through the ScalingLayer -> bf16 [N*H*W][96] = [hi|hi|lo] of the 32
+ * columns k = tap*3 + c (27 used), the A operand of conv1_1 (K = 96). */
+int vtp_lpips_prep3(const float* img, void* out_bf16, int N, int H, int W, vtp_stream_t stream);
+/* nn.MaxPool2d(2,2) on NHWC fp32 */
+int vtp_maxpool2_f32(const float* x, float* y, int B, int H, int W, int C, vtp_stream_t stream);
+/* one tap of the metric (lpips.py:88-100): f fp32 NHWC [2n][HW][C] holds n (reference, reconstruction) pairs
+ * interleaved; part[i*ldp + col0 + s] = (1/HW) * sum over slice s of image pair i's pixels of
+ * sum_c w_c (f0_c / (||f0|| + 1e-10) - f1_c / (||f1|| + 1e-10))^2, s < slices.  No atomics. */
+int vtp_lpips_tap_metric(const float* f, const float* w, int n, int HW, int C, double* part, int ldp, int col0, int slices,
+                         vtp_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Contrastive exchange over NVLink peer memory (vtp_b200/csrc/clip.cu): collective C2 of SURVEY.md §8e — the feature
@@ -332,6 +344,35 @@ int vtp_probe_sgd(float* p, const float* g, float* buf, long n, int row_len, int
  * rules (first maximal index; NaN counts as the maximum, the first NaN wins). */
 int vtp_probe_correct(const float* Z, long ldz, int B, int G, int C, int Cp, const int64_t* labels, int64_t* counts,
                       vtp_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------------------
+ * Reconstruction metrics (vtp_b200/csrc/recon_metrics.cu): tools/test_reconstruction_hf.py:371-402 over one batch of
+ * B pairs, x = the ImageNet-normalised input (fp32 NCHW [B][3][H][W]) and rec = the decoder output (fp32 | bf16, same
+ * shape).  Both are denormalised as (v - sub3[c]) / div3[c] in fp32 and clamped to [0, 1] (o, r below).  No atomics:
+ * repeated runs are bit-identical.
+ * ------------------------------------------------------------------------------------------------------------ */
+/* One pass over both images.  u8_ref / u8_rec (optional, both or neither): uint8 NHWC [B][H][W][3] = trunc(o*255),
+ * trunc(r*255) (:401-402, bit-identical with vtp_image_to_u8); lp (optional): fp32 NCHW [B][2][3][H][W], the LPIPS
+ * network input ((v*2 - 1) - shift) / scale of o (slot 0) and r (slot 1); sse_part fp64 [B][nbands]: sum over band j
+ * (rows [j*ceil(H/nbands), ...); a band past the last row sums to 0) of (o*255 - r*255)^2, the fp32 difference
+ * squared in fp64.  B, nbands <= 65535. */
+int vtp_recon_pixels(const float* x, const void* rec, int rec_dtype, int B, int H, int W, const float* sub3,
+                     const float* div3, uint8_t* u8_ref, uint8_t* u8_rec, float* lp, double* sse_part, int nbands,
+                     vtp_stream_t stream);
+/* torchmetrics StructuralSimilarityIndexMeasure(data_range=1) (:392): 11x11 Gaussian window (sigma 1.5), C1 = 0.01^2,
+ * C2 = 0.03^2, variances clamped at 0, over the 3*(H-10)*(W-10) windows wholly inside the image (the reflect-padded map
+ * with its 5-pixel border cropped).  part fp64 [B][vtp_recon_ssim_tiles(H, W)]: per-tile sums of the SSIM map.
+ * H, W >= 11. */
+int vtp_recon_ssim(const float* x, const void* rec, int rec_dtype, int B, int H, int W, const float* sub3,
+                   const float* div3, double* part, vtp_stream_t stream);
+/* number of SSIM tiles per image (0 if H or W < 11); launches nothing */
+int vtp_recon_ssim_tiles(int H, int W);
+/* Per image, partials summed in ascending order: psnr[b] (fp64) = 20 log10(255 / sqrt(sse / (3HW))) (+inf when
+ * sse == 0, :49-62), ssim[b] = SSIM-map sum / (3 (H-10)(W-10)), lpips[b] = sum of lp_part[b][0..nlp) (if lp_part is given,
+ * vtp_lpips_tap_metric's partials).  Then acc (fp64, device) += {sum_b psnr, B, mean_b ssim, mean_b lpips, 1}. */
+int vtp_recon_finalise(const double* sse_part, int nbands, const double* ssim_part, int ntiles, const double* lp_part,
+                       int nlp, int B, int H, int W, double* psnr, float* ssim, float* lpips, double* acc,
+                       vtp_stream_t stream);
 
 #ifdef __cplusplus
 }

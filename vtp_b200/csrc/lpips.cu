@@ -230,6 +230,98 @@ __global__ void lpips_img_grad_kernel(const __nv_bfloat16* __restrict__ dcol, fl
     }
 }
 
+// ---------------------------------------------------------------- fp32-accurate metric forward (bf16x3 operands)
+// img fp32 NCHW [N][3][H][W], already through the ScalingLayer -> out bf16 [N*H*W][96] = [hi|hi|lo] of the 3x3 im2col
+// (k = tap*3 + c, 27 values padded to 32): the A operand of conv1_1 against [hi|lo|hi] weights (K = 96).
+__global__ void lpips_prep3_kernel(const float* __restrict__ img, __nv_bfloat16* __restrict__ out, int N, int H, int W) {
+    const long P = (long)N * H * W;
+    for (long pix = blockIdx.x * (long)blockDim.x + threadIdx.x; pix < P; pix += (long)gridDim.x * blockDim.x) {
+        const int w = (int)(pix % W), h = (int)((pix / W) % H);
+        const long b = pix / ((long)W * H);
+        float vals[32];
+#pragma unroll
+        for (int tap = 0; tap < 9; ++tap) {
+            const int hh = h + tap / 3 - 1, ww = w + tap % 3 - 1;
+            const bool in = hh >= 0 && hh < H && ww >= 0 && ww < W;
+#pragma unroll
+            for (int c = 0; c < 3; ++c) vals[tap * 3 + c] = in ? __ldg(img + ((b * 3 + c) * H + hh) * W + ww) : 0.f;
+        }
+#pragma unroll
+        for (int i = 27; i < 32; ++i) vals[i] = 0.f;
+        uint32_t hi[16], lo[16];
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+            const float h0 = bf16_round(vals[2 * i]), h1 = bf16_round(vals[2 * i + 1]);
+            hi[i] = pack_bf16x2(h0, h1);
+            lo[i] = pack_bf16x2(vals[2 * i] - h0, vals[2 * i + 1] - h1);
+        }
+        uint4* o = reinterpret_cast<uint4*>(out + pix * 96);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            o[i] = make_uint4(hi[4 * i], hi[4 * i + 1], hi[4 * i + 2], hi[4 * i + 3]);
+            o[4 + i] = o[i];
+            o[8 + i] = make_uint4(lo[4 * i], lo[4 * i + 1], lo[4 * i + 2], lo[4 * i + 3]);
+        }
+    }
+}
+
+// nn.MaxPool2d(2,2) on fp32 NHWC, 4 channels per thread
+__global__ void maxpool2_f32_kernel(const float* __restrict__ x, float* __restrict__ y, int B, int H, int W, int C) {
+    const int Ho = H / 2, Wo = W / 2, C4 = C / 4;
+    const long total = (long)B * Ho * Wo * C4;
+    for (long t = blockIdx.x * (long)blockDim.x + threadIdx.x; t < total; t += (long)gridDim.x * blockDim.x) {
+        const int c = (int)(t % C4) * 4;
+        const long pix = t / C4;
+        const int wo = (int)(pix % Wo), ho = (int)((pix / Wo) % Ho);
+        const long b = pix / ((long)Wo * Ho);
+        const float* p0 = x + ((b * H + 2 * ho) * W + 2 * wo) * C + c;
+        const float4 a = __ldg(reinterpret_cast<const float4*>(p0)), q = __ldg(reinterpret_cast<const float4*>(p0 + C));
+        const float4 r = __ldg(reinterpret_cast<const float4*>(p0 + (long)W * C));
+        const float4 s = __ldg(reinterpret_cast<const float4*>(p0 + (long)W * C + C));
+        float4 o;
+        o.x = fmaxf(fmaxf(a.x, q.x), fmaxf(r.x, s.x)), o.y = fmaxf(fmaxf(a.y, q.y), fmaxf(r.y, s.y));
+        o.z = fmaxf(fmaxf(a.z, q.z), fmaxf(r.z, s.z)), o.w = fmaxf(fmaxf(a.w, q.w), fmaxf(r.w, s.w));
+        *reinterpret_cast<float4*>(y + pix * C + c) = o;
+    }
+}
+
+// Forward-only LPIPS tap on fp32 NHWC features f [2n][HW][C] with the pairs interleaved (image 2i = reference,
+// 2i + 1 = reconstruction): part[i*ldp + col0 + s] = (1/HW) Σ_{pixels of slice s} Σ_c w_c (f0_c/(‖f0‖+eps) − f1_c/(‖f1‖+eps))².
+// grid (slices, n), one warp per pixel in a fixed assignment, fp64 block sum: no atomics.
+template <int CPL>  // channels per lane (C = 32 * CPL)
+__global__ void __launch_bounds__(256) lpips_tap_metric_kernel(const float* __restrict__ f, const float* __restrict__ w, int HW,
+                                                               double* __restrict__ part, int ldp, int col0) {
+    constexpr int C = 32 * CPL;
+    __shared__ double sh[32];
+    const int i = blockIdx.y, s = blockIdx.x, lane = threadIdx.x & 31;
+    const int warp = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), nwarps = gridDim.x * (blockDim.x >> 5);
+    const float* f0 = f + (long)(2 * i) * HW * C;
+    const float* f1 = f0 + (long)HW * C;
+    float wv[CPL];
+#pragma unroll
+    for (int k = 0; k < CPL; ++k) wv[k] = __ldg(w + k * 32 + lane);
+    double local = 0.0;
+    for (int p = warp; p < HW; p += nwarps) {
+        float a[CPL], bq[CPL], s0 = 0.f, s1 = 0.f;
+#pragma unroll
+        for (int k = 0; k < CPL; ++k) {
+            a[k] = __ldg(f0 + (long)p * C + k * 32 + lane), bq[k] = __ldg(f1 + (long)p * C + k * 32 + lane);
+            s0 = fmaf(a[k], a[k], s0), s1 = fmaf(bq[k], bq[k], s1);
+        }
+        s0 = warp_sum(s0), s1 = warp_sum(s1);
+        const float n0 = sqrtf(s0) + 1e-10f, n1 = sqrtf(s1) + 1e-10f;
+        float d = 0.f;
+#pragma unroll
+        for (int k = 0; k < CPL; ++k) {
+            const float diff = __fdiv_rn(a[k], n0) - __fdiv_rn(bq[k], n1);
+            d = fmaf(wv[k], diff * diff, d);
+        }
+        local += (double)warp_sum(d);  // identical in every lane; lane 0's copy is summed below
+    }
+    const double tot = block_sum_f64(lane == 0 ? local : 0.0, sh);
+    if (threadIdx.x == 0) part[(long)i * ldp + col0 + s] = tot / HW;
+}
+
 static inline int gridn(long n, int block) {
     long g = (n + block - 1) / block;
     long cap = (long)num_sms() * 16;
@@ -282,6 +374,39 @@ extern "C" int vtp_lpips_tap(const void* f0, const void* f1, const float* w, voi
         case 256: lpips_tap_kernel<32, 1><<<gridn(P * 32, 256), 256, 0, stream>>>(a0, a1, w, g, P, coef, loss_acc); break;
         case 512: lpips_tap_kernel<32, 2><<<gridn(P * 32, 256), 256, 0, stream>>>(a0, a1, w, g, P, coef, loss_acc); break;
         default: VTP_FAIL(VTP_ERR_ARG, "lpips_tap: C = %d not in {64, 128, 256, 512}", C);
+    }
+    VTP_LAUNCH_CHECK();
+    return VTP_OK;
+}
+
+extern "C" int vtp_lpips_prep3(const float* img, void* out_bf16, int N, int H, int W, vtp_stream_t st) {
+    VTP_CHECK_ARG(img && out_bf16 && N > 0 && H > 0 && W > 0 && ((uintptr_t)out_bf16 & 15) == 0, "lpips_prep3: bad args");
+    const long P = (long)N * H * W;
+    lpips_prep3_kernel<<<gridn(P, 128), 128, 0, (cudaStream_t)st>>>(img, (__nv_bfloat16*)out_bf16, N, H, W);
+    VTP_LAUNCH_CHECK();
+    return VTP_OK;
+}
+
+extern "C" int vtp_maxpool2_f32(const float* x, float* y, int B, int H, int W, int C, vtp_stream_t st) {
+    VTP_CHECK_ARG(x && y && B > 0 && H % 2 == 0 && W % 2 == 0 && C % 4 == 0, "maxpool2_f32: bad args (even H, W; C %% 4)");
+    const long total = (long)B * (H / 2) * (W / 2) * (C / 4);
+    maxpool2_f32_kernel<<<gridn(total, 256), 256, 0, (cudaStream_t)st>>>(x, y, B, H, W, C);
+    VTP_LAUNCH_CHECK();
+    return VTP_OK;
+}
+
+extern "C" int vtp_lpips_tap_metric(const float* f, const float* w, int n, int HW, int C, double* part, int ldp, int col0,
+                                    int slices, vtp_stream_t st) {
+    VTP_CHECK_ARG(f && w && part && n > 0 && n <= 65535 && HW > 0 && slices > 0 && col0 >= 0 && col0 + slices <= ldp,
+                  "lpips_tap_metric: bad args (col0 + slices <= ldp)");
+    const dim3 grid(slices, n);
+    cudaStream_t stream = (cudaStream_t)st;
+    switch (C) {
+        case 64: lpips_tap_metric_kernel<2><<<grid, 256, 0, stream>>>(f, w, HW, part, ldp, col0); break;
+        case 128: lpips_tap_metric_kernel<4><<<grid, 256, 0, stream>>>(f, w, HW, part, ldp, col0); break;
+        case 256: lpips_tap_metric_kernel<8><<<grid, 256, 0, stream>>>(f, w, HW, part, ldp, col0); break;
+        case 512: lpips_tap_metric_kernel<16><<<grid, 256, 0, stream>>>(f, w, HW, part, ldp, col0); break;
+        default: VTP_FAIL(VTP_ERR_ARG, "lpips_tap_metric: C = %d not in {64, 128, 256, 512}", C);
     }
     VTP_LAUNCH_CHECK();
     return VTP_OK;

@@ -221,5 +221,19 @@ __device__ __forceinline__ float warp_max(float v) {
     for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
     return v;
 }
+// fp64 sum over the block in a fixed order (warp butterflies, then the warps in ascending order); the result is valid
+// in thread 0.  sh: 32 doubles of shared memory.  Every thread of the block must call it.
+__device__ __forceinline__ double block_sum_f64(double v, double* sh) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    __syncthreads();
+    if (lane == 0) sh[warp] = v;
+    __syncthreads();
+    double s = 0.0;
+    if (threadIdx.x == 0)
+        for (int i = 0; i < nw; ++i) s += sh[i];
+    return s;
+}
 
 }  // namespace vtp

@@ -102,6 +102,17 @@ SIGNATURES: dict[str, tuple] = {
     "vtp_lpips_tap": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_long, C.c_int, C.c_float, C.c_void_p,
                                 C.c_void_p]),
     "vtp_lpips_img_grad": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "vtp_lpips_prep3": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "vtp_maxpool2_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "vtp_lpips_tap_metric": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int,
+                                       C.c_int, C.c_void_p]),
+    "vtp_recon_pixels": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "vtp_recon_ssim": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                 C.c_void_p, C.c_void_p]),
+    "vtp_recon_ssim_tiles": (C.c_int, [C.c_int, C.c_int]),
+    "vtp_recon_finalise": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                     C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vtp_recon_l1_grad": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                     C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p]),
     "vtp_clip_gather_logits": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_long,
@@ -424,6 +435,121 @@ def lpips_tap(f0, f1, w, g0, P: int, Cc: int, coef: float, loss_acc, stream=None
 
 def lpips_img_grad(dcol, dimg, B: int, H: int, W: int, stream=None):
     check(load().vtp_lpips_img_grad(_ptr(dcol), _ptr(dimg), B, H, W, _st(stream)), "vtp_lpips_img_grad")
+
+
+def _need(name: str, t, dtype, shape=None):
+    """Raise unless t is a contiguous CUDA tensor of dtype (and shape)."""
+    if t.dtype != dtype or not t.is_cuda or not t.is_contiguous() or (shape is not None and tuple(t.shape) != tuple(shape)):
+        want = f"[{', '.join(map(str, shape))}]" if shape is not None else ""
+        raise VtpError(f"{name} must be a contiguous CUDA {dtype} tensor {want}, got {t.dtype} {tuple(t.shape)} "
+                       f"on {t.device}")
+
+
+def lpips_prep3(img, out, stream=None):
+    """img fp32 NCHW [N,3,H,W] (ScalingLayer applied) -> out bf16 [N*H*W, 96] (conv1_1's bf16x3 im2col operand)."""
+    import torch
+
+    N, _, H, W = img.shape
+    _need("lpips_prep3: img", img, torch.float32, (N, 3, H, W))
+    _need("lpips_prep3: out", out, torch.bfloat16, (N * H * W, 96))
+    check(load().vtp_lpips_prep3(_ptr(img), _ptr(out), N, H, W, _st(stream)), "vtp_lpips_prep3")
+
+
+def maxpool2_f32(x, y, B: int, H: int, W: int, Cc: int, stream=None):
+    import torch
+
+    _need("maxpool2_f32: x", x, torch.float32)
+    _need("maxpool2_f32: y", y, torch.float32)
+    if x.numel() != B * H * W * Cc or y.numel() != B * (H // 2) * (W // 2) * Cc:
+        raise VtpError(f"maxpool2_f32: sizes of x {tuple(x.shape)} / y {tuple(y.shape)} do not match B,H,W,C = {B, H, W, Cc}")
+    check(load().vtp_maxpool2_f32(_ptr(x), _ptr(y), B, H, W, Cc, _st(stream)), "vtp_maxpool2_f32")
+
+
+def lpips_tap_metric(f, w, n: int, HW: int, Cc: int, part, col0: int, slices: int, stream=None):
+    """f fp32 NHWC [2n, HW, C] (pairs interleaved), w fp32 [C]; part fp64 [n, ldp] receives columns col0 .. col0+slices."""
+    import torch
+
+    _need("lpips_tap_metric: f", f, torch.float32)
+    _need("lpips_tap_metric: w", w, torch.float32, (Cc,))
+    if not part.is_cuda or f.numel() != 2 * n * HW * Cc or part.dtype != torch.float64 or part.dim() != 2 \
+            or part.shape[0] < n or part.stride(1) != 1:
+        raise VtpError("lpips_tap_metric: f must hold 2n*HW*C values and part be a CUDA fp64 [>= n, ldp] tensor with "
+                       "unit column stride")
+    check(load().vtp_lpips_tap_metric(_ptr(f), _ptr(w), n, HW, Cc, _ptr(part), part.stride(0), col0, slices, _st(stream)),
+          "vtp_lpips_tap_metric")
+
+
+# ------------------------------------------------------------------------------------------------ reconstruction metrics
+def recon_ssim_tiles(H: int, W: int) -> int:
+    return int(load().vtp_recon_ssim_tiles(H, W))
+
+
+def _check_pair(what, x, rec, sub3, div3):
+    import torch
+
+    _need(f"{what}: sub3", sub3, torch.float32, (3,))
+    _need(f"{what}: div3", div3, torch.float32, (3,))
+    if x.dim() != 4 or x.shape[1] != 3:
+        raise VtpError(f"{what}: x must be [B,3,H,W], got {tuple(x.shape)}")
+    _need(f"{what}: x", x, torch.float32)
+    if rec.dtype not in (torch.float32, torch.bfloat16) or not rec.is_cuda or not rec.is_contiguous() \
+            or rec.shape != x.shape:
+        raise VtpError(f"{what}: rec must be a contiguous CUDA fp32/bf16 tensor of shape {tuple(x.shape)}, "
+                       f"got {rec.dtype} {tuple(rec.shape)}")
+
+
+def recon_pixels(x, rec, sub3, div3, sse_part, *, u8_ref=None, u8_rec=None, lp=None, stream=None):
+    """See include/vtp_b200.h: x fp32 / rec fp32|bf16 [B,3,H,W]; sse_part fp64 [B, nbands]; u8_* uint8 [B,H,W,3];
+    lp fp32 [B,2,3,H,W]."""
+    import torch
+
+    _check_pair("recon_pixels", x, rec, sub3, div3)
+    B, _, H, W = x.shape
+    _need("recon_pixels: sse_part", sse_part, torch.float64)
+    if sse_part.dim() != 2 or sse_part.shape[0] != B:
+        raise VtpError(f"recon_pixels: sse_part must be [B={B}, nbands], got {tuple(sse_part.shape)}")
+    if (u8_ref is None) != (u8_rec is None):
+        raise VtpError("recon_pixels: give both uint8 outputs or neither")
+    if u8_ref is not None:
+        _need("recon_pixels: u8_ref", u8_ref, torch.uint8, (B, H, W, 3))
+        _need("recon_pixels: u8_rec", u8_rec, torch.uint8, (B, H, W, 3))
+    if lp is not None:
+        _need("recon_pixels: lp", lp, torch.float32, (B, 2, 3, H, W))
+    check(load().vtp_recon_pixels(_ptr(x), _ptr(rec), _dt(rec), B, H, W, _ptr(sub3), _ptr(div3), _ptr(u8_ref), _ptr(u8_rec),
+                                  _ptr(lp), _ptr(sse_part), sse_part.shape[1], _st(stream)), "vtp_recon_pixels")
+
+
+def recon_ssim(x, rec, sub3, div3, part, stream=None):
+    """part fp64 [B, recon_ssim_tiles(H, W)]."""
+    import torch
+
+    _check_pair("recon_ssim", x, rec, sub3, div3)
+    B, _, H, W = x.shape
+    _need("recon_ssim: part", part, torch.float64, (B, recon_ssim_tiles(H, W)))
+    check(load().vtp_recon_ssim(_ptr(x), _ptr(rec), _dt(rec), B, H, W, _ptr(sub3), _ptr(div3), _ptr(part), _st(stream)),
+          "vtp_recon_ssim")
+
+
+def recon_finalise(sse_part, ssim_part, lp_part, H: int, W: int, psnr, ssim, lpips, acc, stream=None):
+    """psnr fp64 [B]; ssim / lpips fp32 [B] (lpips only with lp_part fp64 [B, nlp]); acc fp64 [>= 5] (device)."""
+    import torch
+
+    B = sse_part.shape[0]
+    _need("recon_finalise: sse_part", sse_part, torch.float64)
+    _need("recon_finalise: ssim_part", ssim_part, torch.float64, (B, recon_ssim_tiles(H, W)))
+    _need("recon_finalise: psnr", psnr, torch.float64, (B,))
+    _need("recon_finalise: ssim", ssim, torch.float32, (B,))
+    _need("recon_finalise: acc", acc, torch.float64)
+    if lp_part is not None:
+        _need("recon_finalise: lp_part", lp_part, torch.float64)
+        if lp_part.dim() != 2 or lp_part.shape[0] != B:
+            raise VtpError(f"recon_finalise: lp_part must be [B={B}, nlp], got {tuple(lp_part.shape)}")
+        _need("recon_finalise: lpips", lpips, torch.float32, (B,))
+    if acc.numel() < 5:
+        raise VtpError("recon_finalise: acc needs 5 fp64 slots")
+    check(load().vtp_recon_finalise(_ptr(sse_part), sse_part.shape[1], _ptr(ssim_part), ssim_part.shape[1], _ptr(lp_part),
+                                    lp_part.shape[1] if lp_part is not None else 0, B, H, W, _ptr(psnr), _ptr(ssim),
+                                    _ptr(lpips), _ptr(acc), _st(stream)), "vtp_recon_finalise")
 
 
 def swiglu_fwd(pre, hid, M: int, Hs: int, stream=None):

@@ -3,7 +3,11 @@
 Mirrors the reference's metric module vtp/utils/lpips.py:61-171 (ScalingLayer -> VGG16 features, 5 ReLU taps ->
 channel unit-normalise -> squared difference -> 1x1 `lin` -> spatial mean -> sum).  The reference downloads the VGG16 /
 lin weights at run time (lpips.py:15-17,48-58,130) which is impossible offline: weights are supplied by the caller
-(`from_tensors`) or drawn from a seeded generator (`random_init`, He-normal convs, positive lin weights) — SURVEY.md §7.
+(the constructors' tensor lists, or `LPIPSMetric.from_files`) or drawn from a seeded generator (`random_init`, He-normal
+convs, positive lin weights) — SURVEY.md §7.
+
+`LPIPSLoss` is the bf16 training loss (value + gradient); `LPIPSMetric` is the fp32-accurate, forward-only evaluation
+metric of the reconstruction evaluator (vtp_b200/recon_eval.py).
 
 All 13 3x3 convolutions and their input-gradients run on the wgmma GEMM in implicit-conv mode (4-D TMA over NHWC
 bf16 activations, zero fill = padding; bias+ReLU, respectively the ReLU mask, fused in the epilogue); conv1_1 (3 input
@@ -148,6 +152,131 @@ class LPIPSLoss:
         dcol = _e((M, 32), BF, dev)
         lib.gemm(dz, self.w_fwd[0], dcol, M=M, N=32, K=64, lda=64, ldb=32, b_mn=True, ldo=32, round_bf16=False)
         lib.lpips_img_grad(dcol, dimg, B, h, w)
+
+
+VGG_FEATURE_INDEX = (0, 2, 5, 7, 10, 12, 14, 17, 19, 21, 24, 26, 28)  # torchvision vgg16.features index of each conv
+
+
+class LPIPSMetric:
+    """The reference's LPIPS module as an evaluation metric (tools/test_reconstruction_hf.py:379-388): per-image values,
+    forward only, fp32-accurate.  The reference runs the VGG in fp32 (TF32 convolutions under cuDNN's default); here
+    every conv is the implicit-conv wgmma GEMM on bf16x3 operands (activations [hi|hi|lo] over 3C channels, weights
+    [hi|lo|hi] per tap, fp32 accumulation and output with bias + ReLU), max-pool runs in fp32, and only the five taps
+    are kept.  Images are processed in chunks of `chunk` pairs to bound activation memory.
+
+    Shapes: the conv GEMM needs every feature map's width to be a multiple of 4, so H % 16 == 0 and W % 64 == 0."""
+
+    def __init__(self, vgg_w: Sequence[torch.Tensor], vgg_b: Sequence[torch.Tensor], lin_w: Sequence[torch.Tensor],
+                 device="cuda", chunk: int = 8):
+        """vgg_w[i]: [Cout, Cin, 3, 3], vgg_b[i]: [Cout], lin_w[k]: [1, C_k, 1, 1] (torch layouts, 13 convs, 5 lins)."""
+        if len(vgg_w) != 13 or len(vgg_b) != 13 or len(lin_w) != 5:
+            raise ValueError(f"LPIPSMetric: 13 conv weights / biases and 5 lin weights expected, got "
+                             f"{len(vgg_w)} / {len(vgg_b)} / {len(lin_w)}")
+        self.device, self.chunk = torch.device(device), int(chunk)
+        dev = self.device
+        self.cin = [int(w.shape[1]) for w in vgg_w]
+        self.cout = [int(w.shape[0]) for w in vgg_w]
+        self.w3, self.bias = [], []
+        for i, (w, b) in enumerate(zip(vgg_w, vgg_b)):
+            w = w.to(dev, F32)
+            co, ci = w.shape[0], w.shape[1]
+            if i == 0:  # [64, 27 -> 32] (k = tap*3 + c) -> [64, 96] = [hi|lo|hi]
+                wf = torch.zeros(co, 32, device=dev)
+                wf[:, :27] = w.permute(0, 2, 3, 1).reshape(co, 27)
+                w3 = _e((co, 96), BF, dev)
+                lib.split3(wf, w3, co, 32, b_side=True)
+            else:  # [Cout, 9, Cin] -> [Cout, 9 * 3Cin]: per tap [hi|lo|hi] of Cin
+                wt = w.permute(0, 2, 3, 1).reshape(co * 9, ci).contiguous()
+                w3 = _e((co, 9 * 3 * ci), BF, dev)
+                lib.split3(wt, w3, co * 9, ci, b_side=True)
+            self.w3.append(w3)
+            self.bias.append(b.to(dev, F32).contiguous())
+        self.lin = [l.to(dev, F32).reshape(-1).contiguous() for l in lin_w]
+
+    @classmethod
+    def random_init(cls, seed: int = 0, device="cuda", chunk: int = 8) -> "LPIPSMetric":
+        vw, vb, lw = random_weights(seed)
+        return cls(vw, vb, lw, device=device, chunk=chunk)
+
+    @classmethod
+    def from_files(cls, vgg16_path: str, lin_path: str, device="cuda", chunk: int = 8) -> "LPIPSMetric":
+        """torchvision's VGG16 checkpoint (keys features.{0,2,...,28}.{weight,bias}; the classifier is ignored) and the
+        LPIPS lin file (keys lin{0..4}.model.1.weight; other keys are ignored, as the reference's strict=False load)."""
+        return cls(*load_weight_files(vgg16_path, lin_path), device=device, chunk=chunk)
+
+    @staticmethod
+    def check_shape(H: int, W: int) -> None:
+        if H % 16 or W % 64:
+            raise ValueError(f"LPIPSMetric: {H}x{W} images are not supported (needs H % 16 == 0 and W % 64 == 0)")
+
+    def parts(self, lp: torch.Tensor) -> torch.Tensor:
+        """lp fp32 [B, 2, 3, H, W] (the ScalingLayer outputs of each (reference, reconstruction) pair, as
+        vtp_recon_pixels writes them) -> fp64 [B, 5 * slices] partials whose row sums are the per-image LPIPS values."""
+        B, _, _, H, W = lp.shape
+        self.check_shape(H, W)
+        part = torch.empty((B, 5 * self.SLICES), dtype=torch.float64, device=lp.device)
+        for s in range(0, B, self.chunk):
+            e = min(B, s + self.chunk)
+            self._chunk(lp[s:e].reshape(2 * (e - s), 3, H, W), part[s:e])
+        return part
+
+    SLICES = 32  # pixel slices per (pair, tap) in the partial sums: 32 CTAs per pair keep a chunk's taps spread over the SMs
+
+    def _chunk(self, img: torch.Tensor, part: torch.Tensor) -> None:
+        dev = img.device
+        N, _, H, W = img.shape
+        n = N // 2
+        col = _e((N * H * W, 96), BF, dev)
+        lib.lpips_prep3(img, col)
+        x, h, w, ci, k = None, H, W, 0, 0
+        for c in VGG_CFG:
+            if c == "M":
+                y = _e((N, h // 2, w // 2, x.shape[-1]), F32, dev)
+                lib.maxpool2_f32(x, y, N, h, w, x.shape[-1])
+                x, h, w = y, h // 2, w // 2
+                continue
+            y = _e((N, h, w, c), F32, dev)
+            M = N * h * w
+            if ci == 0:
+                lib.gemm(col, self.w3[0], y, M=M, N=c, K=96, bias=self.bias[0], act=lib.ACT_RELU, ldo=c, round_bf16=False)
+            else:
+                cin = self.cin[ci]
+                a3 = _e((M, 3 * cin), BF, dev)
+                lib.split3(x.view(M, cin), a3, M, cin, b_side=False)
+                lib.gemm(a3, self.w3[ci], y, M=M, N=c, K=27 * cin, lda=3 * cin, ldb=27 * cin, bias=self.bias[ci],
+                         act=lib.ACT_RELU, ldo=c, conv=(3 * cin, h, w), round_bf16=False)
+            if ci in TAPS:
+                lib.lpips_tap_metric(y, self.lin[k], n, h * w, c, part, k * self.SLICES, self.SLICES)
+                k += 1
+            x = y
+            ci += 1
+
+
+def load_weight_files(vgg16_path: str, lin_path: str):
+    """(vgg_w, vgg_b, lin_w) tensor lists from torchvision's VGG16 checkpoint and the LPIPS lin file (CPU tensors).
+    Raises KeyError naming every missing key."""
+    vgg, lin = _load_state(vgg16_path), _load_state(lin_path)
+    need = [f"features.{j}.{p}" for j in VGG_FEATURE_INDEX for p in ("weight", "bias")]
+    missing = [k for k in need if k not in vgg]
+    if missing:
+        raise KeyError(f"{vgg16_path}: missing VGG16 keys {missing}")
+    lneed = [f"lin{k}.model.1.weight" for k in range(5)]
+    missing = [k for k in lneed if k not in lin]
+    if missing:
+        raise KeyError(f"{lin_path}: missing LPIPS lin keys {missing}")
+    return ([vgg[f"features.{j}.weight"] for j in VGG_FEATURE_INDEX], [vgg[f"features.{j}.bias"] for j in VGG_FEATURE_INDEX],
+            [lin[k] for k in lneed])
+
+
+def _load_state(path: str):
+    if path.endswith(".safetensors"):
+        from safetensors.torch import load_file
+
+        return load_file(path)
+    sd = torch.load(path, map_location="cpu", weights_only=True)
+    if isinstance(sd, dict) and "state_dict" in sd and isinstance(sd["state_dict"], dict):
+        sd = sd["state_dict"]
+    return sd
 
 
 def random_weights(seed: int = 0):
