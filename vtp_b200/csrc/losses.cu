@@ -123,8 +123,9 @@ dino_teacher_kernel(__nv_bfloat16* __restrict__ t, const float* __restrict__ cen
     }
 }
 
-// student: for row r with teacher rows t0[r], t1[r] (−1 = none), weight w[r]:
+// student: for row r with teacher rows t0[r], t1[r] (−1 = none; either may be −1, t1 may be NULL), weight w[r]:
 //   z = s/τ ;  loss += w Σ_v (lse(z) − Σ_k T_v[k] z[k]) ;  ds[k] = (w/τ) (n_v softmax(z)[k] − Σ_v T_v[k])   (in place, bf16)
+// A row without teachers gets zero loss and gradient.
 __global__ void __launch_bounds__(1024, 1)
 dino_student_kernel(__nv_bfloat16* __restrict__ s, const __nv_bfloat16* __restrict__ tprobs,
                     const int* __restrict__ t0, const int* __restrict__ t1, const float* __restrict__ w,
@@ -137,6 +138,7 @@ dino_student_kernel(__nv_bfloat16* __restrict__ s, const __nv_bfloat16* __restri
     const float wr = w[r];
     const uint4* ta = i0 >= 0 ? reinterpret_cast<const uint4*>(tprobs + (long)i0 * K) : nullptr;
     const uint4* tb = i1 >= 0 ? reinterpret_cast<const uint4*>(tprobs + (long)i1 * K) : nullptr;
+    if (!ta) ta = tb, tb = nullptr;   // the teacher terms below are read under `if (ta)`: a lone t1 moves to the first slot
     const float nv = (ta ? 1.f : 0.f) + (tb ? 1.f : 0.f);
     const int K8 = K >> 3;
     const float it2 = inv_temp * 1.4426950408889634f;
