@@ -374,6 +374,31 @@ int vtp_recon_finalise(const double* sse_part, int nbands, const double* ssim_pa
                        int nlp, int B, int H, int W, double* psnr, float* ssim, float* lpips, double* acc,
                        vtp_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Zero-shot classification (vtp_b200/csrc/zero_shot.cu): tools/test_zero_shot_hf.py's prompt-ensemble classifier and
+ * top-k accuracy.  The logits GEMM is vtp_gemm_bf16 (bf16x3 with fp32 out, or bf16 with bf16 out).  No atomics except
+ * the integer hit counters: every other output is bit-reproducible.
+ * ------------------------------------------------------------------------------------------------------------ */
+enum { VTP_ZS_MAX_K = 8 };
+/* build_zero_shot_classifier (:374-385) from per-prompt text features feat [rows][E] (fp32 | bf16, as the text tower
+ * returned them).  Prompt (c, t) is row row_of[c*T + t] (int32, optional: row c*T + t without it).  Per prompt
+ * f = x / max(||x||, 1e-12) in fp32 (F.normalize under CUDA autocast: fp32 norm, fp32 division); per class the mean of
+ * its T rows, summed in ascending t, divided by T and normalised the same way.  out fp32 [Cp][E]: row c < C is class c,
+ * rows C..Cp-1 are 0.  One CTA per row of out; E <= 1024. */
+int vtp_zs_class_embed(const void* feat, int feat_dtype, const int* row_of, int C, int T, int E, int Cp, float* out,
+                       vtp_stream_t stream);
+/* evaluate's image side (:431-432) from the UNNORMALISED image features x [B][E] (fp32 | bf16):
+ * out = fl32(scale * fl32(x / max(||x||, 1e-12))) with an fp32 norm, written fp32 or rounded once to bf16 (autocast's
+ * cast of the matmul operand).  One warp per row. */
+int vtp_zs_image_operand(const void* x, int x_dtype, int B, int E, float scale, void* out, int out_dtype,
+                         vtp_stream_t stream);
+/* accuracy (:312-316) through each target's rank.  logits [B][ld] (fp32 | bf16), C valid columns, int64 targets [B]:
+ * ranks[b] = #{j : l_j ahead of l_t} with "ahead" = NaN above every number, then larger value, then (equal values,
+ * or both NaN) lower index; a target outside [0, C) gets rank C.  counts[i] (int64) += #{b : ranks[b] < ks[i]} for
+ * the nk <= VTP_ZS_MAX_K values ks (host array, read at launch).  One warp per row. */
+int vtp_zs_rank(const void* logits, int dtype, long ld, int B, int C, const int64_t* targets, const int* ks, int nk,
+                int* ranks, int64_t* counts, vtp_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

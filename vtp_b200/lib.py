@@ -143,6 +143,11 @@ SIGNATURES: dict[str, tuple] = {
                                 C.c_int, C.c_void_p, C.c_float, C.c_float, C.c_void_p, C.c_void_p]),
     "vtp_probe_correct": (C.c_int, [C.c_void_p, C.c_long, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                     C.c_void_p]),
+    "vtp_zs_class_embed": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                     C.c_void_p]),
+    "vtp_zs_image_operand": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_int, C.c_void_p]),
+    "vtp_zs_rank": (C.c_int, [C.c_void_p, C.c_int, C.c_long, C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_int), C.c_int,
+                              C.c_void_p, C.c_void_p, C.c_void_p]),
 }
 
 
@@ -637,6 +642,72 @@ def probe_sgd(p, g, buf, n: int, *, row_len: int, rows_per_cls: int, cls0: int, 
 def probe_correct(Z, B: int, G: int, Cn: int, Cp: int, labels, counts, stream=None):
     check(load().vtp_probe_correct(_ptr(Z), Z.stride(0), B, G, Cn, Cp, _ptr(labels), _ptr(counts), _st(stream)),
           "vtp_probe_correct")
+
+
+# ------------------------------------------------------------------------------------------------ zero-shot classification
+ZS_MAX_K = 8
+
+
+def _need_float(name: str, t, shape=None):
+    import torch
+
+    if t.dtype not in (torch.float32, torch.bfloat16) or not t.is_cuda or not t.is_contiguous() \
+            or (shape is not None and tuple(t.shape) != tuple(shape)):
+        raise VtpError(f"{name} must be a contiguous CUDA fp32/bf16 tensor{'' if shape is None else ' ' + str(list(shape))}"
+                       f", got {t.dtype} {tuple(t.shape)} on {t.device}")
+
+
+def zs_class_embed(feat, out, C: int, T: int, row_of=None, stream=None):
+    """feat fp32|bf16 [rows, E] (per-prompt text features); row_of int32 [C*T] (prompt c*T + t -> row) or None (rows in
+    class-major order); out fp32 [Cp >= C, E] <- normalised template means, padding rows 0."""
+    import torch
+
+    _need_float("zs_class_embed: feat", feat)
+    if feat.dim() != 2:
+        raise VtpError(f"zs_class_embed: feat must be [rows, E], got {tuple(feat.shape)}")
+    E = feat.shape[1]
+    _need("zs_class_embed: out", out, torch.float32)
+    if out.dim() != 2 or out.shape[1] != E or out.shape[0] < C:
+        raise VtpError(f"zs_class_embed: out must be fp32 [>= {C}, {E}], got {tuple(out.shape)}")
+    if row_of is not None:
+        _need("zs_class_embed: row_of", row_of, torch.int32, (C * T,))
+    elif feat.shape[0] < C * T:
+        raise VtpError(f"zs_class_embed: {feat.shape[0]} feature rows for C*T = {C * T} prompts")
+    check(load().vtp_zs_class_embed(_ptr(feat), _dt(feat), _ptr(row_of), C, T, E, out.shape[0], _ptr(out), _st(stream)),
+          "vtp_zs_class_embed")
+
+
+def zs_image_operand(x, out, scale: float = 100.0, stream=None):
+    """out[b] = scale * x[b] / max(||x[b]||, 1e-12) in fp32 (out fp32, or bf16 rounded once).  x fp32|bf16 [B, E]."""
+    _need_float("zs_image_operand: x", x)
+    if x.dim() != 2:
+        raise VtpError(f"zs_image_operand: x must be [B, E], got {tuple(x.shape)}")
+    _need_float("zs_image_operand: out", out, tuple(x.shape))
+    B, E = x.shape
+    check(load().vtp_zs_image_operand(_ptr(x), _dt(x), B, E, scale, _ptr(out), _dt(out), _st(stream)),
+          "vtp_zs_image_operand")
+
+
+def zs_rank(logits, Cn: int, targets, ranks, counts=None, ks=(), stream=None):
+    """ranks int32 [B] <- rank of each row's target among the first Cn logits (NaN first, ties to the lower index;
+    Cn for a target outside [0, Cn)); counts int64 [len(ks)] += #{rank < k}.  logits fp32|bf16 [B, ld >= Cn]."""
+    import torch
+
+    if logits.dtype not in (torch.float32, torch.bfloat16) or not logits.is_cuda or logits.dim() != 2 \
+            or logits.stride(1) != 1 or logits.shape[1] < Cn:
+        raise VtpError(f"zs_rank: logits must be a CUDA fp32/bf16 [B, >= {Cn}] tensor with unit column stride, got "
+                       f"{logits.dtype} {tuple(logits.shape)}")
+    B = logits.shape[0]
+    _need("zs_rank: targets", targets, torch.int64, (B,))
+    _need("zs_rank: ranks", ranks, torch.int32, (B,))
+    ks = [int(k) for k in ks]
+    if len(ks) > ZS_MAX_K:
+        raise VtpError(f"zs_rank: at most {ZS_MAX_K} values of k, got {len(ks)}")
+    if ks:
+        _need("zs_rank: counts", counts, torch.int64, (len(ks),))
+    karr = (C.c_int * max(1, len(ks)))(*ks)
+    check(load().vtp_zs_rank(_ptr(logits), _dt(logits), logits.stride(0), B, Cn, _ptr(targets), karr, len(ks), _ptr(ranks),
+                             _ptr(counts) if ks else None, _st(stream)), "vtp_zs_rank")
 
 
 # ------------------------------------------------------------------------------------------------ image / latent formats
