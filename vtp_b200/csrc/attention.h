@@ -12,7 +12,7 @@ struct AttnDev {
     const __nv_bfloat16* qkv;  // [B*T][3D]
     __nv_bfloat16* out;        // [B*T][D]
     float* lse;                // [B][H][T] or null
-    int B, T, H, D, prefix, HW, causal, nkt;  // nkt = number of 128-key tiles (1|2)
+    int B, T, H, D, prefix, HW, causal;
     int pack;  // > 0: `pack` whole sequences (T <= 64 tokens, prefix tokens included as ordinary rows) share one 128-row tile
     float scale_log2;                         // scale * log2(e)
     float scale;
