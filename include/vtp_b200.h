@@ -399,6 +399,34 @@ int vtp_zs_image_operand(const void* x, int x_dtype, int B, int E, float scale, 
 int vtp_zs_rank(const void* logits, int dtype, long ld, int B, int C, const int64_t* targets, const int* ks, int nk,
                 int* ranks, int64_t* counts, vtp_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Fréchet Inception Distance (vtp_b200/csrc/fid.cu): pytorch-fid's calculate_fid_given_paths(dims = 2048), called by
+ * tools/test_reconstruction_hf.py:98-104 for rFID.  The 94 convolutions are vtp_gemm_bf16 on bf16x3 operands with fp32
+ * output (BN folded into weights and bias, ReLU in the epilogue).  Activations are fp32 NHWC.  No atomics: every output
+ * is bit-reproducible.
+ * ------------------------------------------------------------------------------------------------------------ */
+/* uint8 NHWC [B][H][W][3] -> fp32 NHWC [B][299][299][3]: ToTensor's /255 (as torch's CUDA x / 255: x * fl(1/255)),
+ * F.interpolate(size = (299, 299), mode = 'bilinear', align_corners = False) with upsample_bilinear2d's fp32
+ * arithmetic (down-sampling too), then 2x - 1.  Any H, W >= 1. */
+int vtp_fid_resize(const uint8_t* u8, int B, int H, int W, float* out, vtp_stream_t stream);
+/* im2col of fp32 NHWC in [B][H][W][ld_in] (channels c0 .. c0+C) for a kh x kw conv with stride and zero padding
+ * (ph, pw) -> the bf16x3 A operand out [B*Ho*Wo][kh*kw*3C]: per tap [hi | hi | lo] of the C channels, against the
+ * [hi | lo | hi] per-tap weights of vtp_split3(b_side = 1).  C = 3 (the stem, 3x3 only): out [B*Ho*Wo][96], the 27
+ * values k = tap*3 + c padded to 32, then [hi | hi | lo].  Otherwise C, ld_in, c0 % 4 == 0. */
+int vtp_fid_im2col3(const float* in, long ld_in, int c0, int B, int H, int W, int C, int kh, int kw, int stride, int ph,
+                    int pw, void* out_bf16, vtp_stream_t stream);
+/* 3x3 pools of fp32 NHWC in [B][H][W][ld_in] (channels 0 .. C) into channels c0 .. c0+C of out [B][Ho][Wo][ld_out]:
+ * mode 0 max, stride 2, no padding; 1 max, stride 1, pad 1; 2 average, stride 1, pad 1, count_include_pad = False
+ * (taps summed row by row).  C, ld_in, ld_out, c0 % 4 == 0. */
+int vtp_fid_pool(const float* in, long ld_in, int B, int H, int W, int C, int mode, float* out, long ld_out, int c0,
+                 vtp_stream_t stream);
+/* x fp32 [B][P][D] (the last block's output, P pixels): f_b = the spatial mean (fp32, pixels summed in order, then
+ * divided by P).  For b < *rows (device int, clamped to [0, B]): S1 (fp64 [D]) += f_b, S2 (fp64 [D][D], upper
+ * triangle by 64x64 tiles) += f_b f_bᵀ, *n += rows.  feat (fp32 [B][D], optional) <- f_b for every b < B.
+ * One CTA per S2 tile, images in order.  D % 64 == 0. */
+int vtp_fid_moments(const float* x, int B, int P, int D, const int* rows, float* feat, double* S2, double* S1, double* n,
+                    vtp_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

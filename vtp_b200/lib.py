@@ -148,6 +148,13 @@ SIGNATURES: dict[str, tuple] = {
     "vtp_zs_image_operand": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_int, C.c_void_p]),
     "vtp_zs_rank": (C.c_int, [C.c_void_p, C.c_int, C.c_long, C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_int), C.c_int,
                               C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vtp_fid_resize": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "vtp_fid_im2col3": (C.c_int, [C.c_void_p, C.c_long, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                  C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "vtp_fid_pool": (C.c_int, [C.c_void_p, C.c_long, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_long,
+                               C.c_int, C.c_void_p]),
+    "vtp_fid_moments": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                  C.c_void_p, C.c_void_p]),
 }
 
 
@@ -708,6 +715,91 @@ def zs_rank(logits, Cn: int, targets, ranks, counts=None, ks=(), stream=None):
     karr = (C.c_int * max(1, len(ks)))(*ks)
     check(load().vtp_zs_rank(_ptr(logits), _dt(logits), logits.stride(0), B, Cn, _ptr(targets), karr, len(ks), _ptr(ranks),
                              _ptr(counts) if ks else None, _st(stream)), "vtp_zs_rank")
+
+
+# ------------------------------------------------------------------------------------------------ FID
+FID_SIZE = 299
+FID_POOL_MAX2, FID_POOL_MAX1, FID_POOL_AVG1 = 0, 1, 2   # vtp_fid_pool modes (see include/vtp_b200.h)
+
+
+def _need_slice(name: str, t, dtype, B: int, H: int, W: int):
+    """t: a contiguous CUDA tensor of dtype, viewed as NHWC [B, H, W, ld]; returns ld."""
+    if t.dtype != dtype or not t.is_cuda or not t.is_contiguous() or t.numel() % (B * H * W) or t.numel() == 0:
+        raise VtpError(f"{name} must be a contiguous CUDA {dtype} tensor of B*H*W = {B * H * W} pixels, got {t.dtype} "
+                       f"{tuple(t.shape)} on {t.device}")
+    return t.numel() // (B * H * W)
+
+
+def fid_resize(u8, out, stream=None):
+    """u8 uint8 NHWC [B,H,W,3] -> out fp32 NHWC [B,299,299,3] = 2 * interpolate(u8 / 255, 299, bilinear) - 1."""
+    import torch
+
+    if u8.dim() != 4 or u8.shape[-1] != 3:
+        raise VtpError(f"fid_resize: u8 must be [B,H,W,3], got {tuple(u8.shape)}")
+    B, H, W, _ = u8.shape
+    _need("fid_resize: u8", u8, torch.uint8)
+    _need("fid_resize: out", out, torch.float32, (B, FID_SIZE, FID_SIZE, 3))
+    check(load().vtp_fid_resize(_ptr(u8), B, H, W, _ptr(out), _st(stream)), "vtp_fid_resize")
+
+
+def fid_conv_out(H: int, W: int, kh: int, kw: int, stride: int, ph: int, pw: int):
+    return (H + 2 * ph - kh) // stride + 1, (W + 2 * pw - kw) // stride + 1
+
+
+def fid_im2col3(x, out, B: int, H: int, W: int, C: int, kernel, stride: int = 1, pad=(0, 0), c0: int = 0, stream=None):
+    """x fp32 NHWC [B,H,W,ld_in] (channels c0 .. c0+C) -> out bf16 [B*Ho*Wo, kh*kw*3C] ([hi|hi|lo] per tap), or
+    [B*Ho*Wo, 96] for the 3-channel stem."""
+    import torch
+
+    kh, kw = kernel
+    ph, pw = pad
+    ld = _need_slice("fid_im2col3: x", x, torch.float32, B, H, W)
+    if c0 < 0 or c0 + C > ld:
+        raise VtpError(f"fid_im2col3: channels {c0}..{c0 + C} outside the {ld} of x")
+    Ho, Wo = fid_conv_out(H, W, kh, kw, stride, ph, pw)
+    if Ho < 1 or Wo < 1:
+        raise VtpError(f"fid_im2col3: a {kh}x{kw} kernel does not fit the padded {H}x{W} input")
+    K = 96 if C == 3 else kh * kw * 3 * C
+    _need("fid_im2col3: out", out, torch.bfloat16, (B * Ho * Wo, K))
+    check(load().vtp_fid_im2col3(_ptr(x), ld, c0, B, H, W, C, kh, kw, stride, ph, pw, _ptr(out), _st(stream)),
+          "vtp_fid_im2col3")
+
+
+def fid_pool(x, out, B: int, H: int, W: int, mode: int, c0: int = 0, stream=None):
+    """3x3 pool of x fp32 NHWC [B,H,W,C] into channels c0 .. c0+C of out fp32 NHWC [B,Ho,Wo,ld_out]."""
+    import torch
+
+    if mode not in (FID_POOL_MAX2, FID_POOL_MAX1, FID_POOL_AVG1):
+        raise VtpError(f"fid_pool: unknown mode {mode}")
+    C = _need_slice("fid_pool: x", x, torch.float32, B, H, W)
+    Ho, Wo = fid_conv_out(H, W, 3, 3, 2, 0, 0) if mode == FID_POOL_MAX2 else (H, W)
+    if Ho < 1 or Wo < 1:
+        raise VtpError(f"fid_pool: a 3x3 stride-2 pool does not fit {H}x{W}")
+    ld = _need_slice("fid_pool: out", out, torch.float32, B, Ho, Wo)
+    if c0 < 0 or c0 + C > ld:
+        raise VtpError(f"fid_pool: channels {c0}..{c0 + C} outside the {ld} of out")
+    check(load().vtp_fid_pool(_ptr(x), C, B, H, W, C, mode, _ptr(out), ld, c0, _st(stream)), "vtp_fid_pool")
+
+
+def fid_moments(x, rows, S2, S1, n, feat=None, stream=None):
+    """x fp32 [B,P,D] (the last block's NHWC output); rows int32 [1] (device); S2 fp64 [D,D], S1 fp64 [D], n fp64 [1]
+    accumulate the images b < rows; feat fp32 [B,D] (optional) <- every image's spatial mean."""
+    import torch
+
+    if x.dim() != 3:
+        raise VtpError(f"fid_moments: x must be [B, P, D], got {tuple(x.shape)}")
+    B, P, D = x.shape
+    if D % 64:
+        raise VtpError(f"fid_moments: D = {D} is not a multiple of 64")
+    _need("fid_moments: x", x, torch.float32)
+    _need("fid_moments: rows", rows, torch.int32, (1,))
+    _need("fid_moments: S2", S2, torch.float64, (D, D))
+    _need("fid_moments: S1", S1, torch.float64, (D,))
+    _need("fid_moments: n", n, torch.float64, (1,))
+    if feat is not None:
+        _need("fid_moments: feat", feat, torch.float32, (B, D))
+    check(load().vtp_fid_moments(_ptr(x), B, P, D, _ptr(rows), _ptr(feat), _ptr(S2), _ptr(S1), _ptr(n), _st(stream)),
+          "vtp_fid_moments")
 
 
 # ------------------------------------------------------------------------------------------------ image / latent formats

@@ -71,7 +71,7 @@ def rank_mean(values_mean: Optional[float], world: int, device) -> Optional[floa
 class _Step:
     """Device buffers of one batch shape (the graph's static inputs and outputs)."""
 
-    def __init__(self, B: int, H: int, W: int, dev, lpips: bool, save: bool):
+    def __init__(self, B: int, H: int, W: int, dev, lpips: bool, save: bool, fid: bool = False):
         self.x = torch.empty((B, 3, H, W), dtype=F32, device=dev)
         self.nbands = min(H, 16)
         self.sse = torch.empty((B, self.nbands), dtype=torch.float64, device=dev)
@@ -81,6 +81,7 @@ class _Step:
         self.lpips = torch.empty(B, dtype=F32, device=dev) if lpips else None
         self.lp = torch.empty((B, 2, 3, H, W), dtype=F32, device=dev) if lpips else None
         self.u8 = torch.empty((2, B, H, W, 3), dtype=torch.uint8, device=dev) if save else None
+        self.fid_rows = torch.zeros(1, dtype=torch.int32, device=dev) if fid else None  # images of the batch with a PNG
         self.graph = None
         self.seen = 0
         self.copied = None   # event: the last PNG copy out of u8 has finished
@@ -94,11 +95,13 @@ class ReconstructionEvaluator:
     reference / reconstruction images are written to save_dir/reference/ref_{i:06d}.png and save_dir/reconstructed/
     rec_{i:06d}.png by a pool of PNG writers fed through pinned buffers on a side stream.  batch_size / world / rank /
     total define the file index as the reference's DistributedSampler loop does (batch_size defaults to the first
-    batch's size, total to no limit)."""
+    batch's size, total to no limit).  fid: an `FIDInception` or None; with it and save_dir, the uint8 reference and
+    reconstruction images that get a PNG also go through the FID network inside the same step (rFID, see vtp_b200/fid.py),
+    so the statistics cover exactly the images the PNG directories hold."""
 
     def __init__(self, model, lpips=None, precision: str = "bf16", save_dir: Optional[str] = None,
                  batch_size: Optional[int] = None, world: Optional[int] = None, rank: Optional[int] = None,
-                 total: Optional[int] = None, use_graph: bool = True, writers: int = 4):
+                 total: Optional[int] = None, use_graph: bool = True, writers: int = 4, fid=None):
         import torch.distributed as dist
 
         if precision not in ("bf16", "fp32"):
@@ -118,6 +121,11 @@ class ReconstructionEvaluator:
         self.acc = torch.zeros(8, dtype=torch.float64, device=dev)
         self.batch_size, self.total = batch_size, total
         self.save_dir = save_dir
+        self.fid = fid if save_dir is not None else None
+        if self.fid is not None:
+            from .fid import FIDStatistics
+
+            self.fid_stats = (FIDStatistics(dev), FIDStatistics(dev))   # reference, reconstruction
         self._steps: Dict[tuple, _Step] = {}
         self._psnr: List[torch.Tensor] = []
         self._ssim: List[torch.Tensor] = []
@@ -152,6 +160,9 @@ class ReconstructionEvaluator:
         lp_part = self.lpips.parts(st.lp) if self.lpips is not None else None
         H, W = st.x.shape[-2:]
         lib.recon_finalise(st.sse, st.ssim_part, lp_part, H, W, st.psnr, st.ssim, st.lpips, self.acc)
+        if self.fid is not None:
+            self.fid.accumulate(st.u8[0], self.fid_stats[0], st.fid_rows)
+            self.fid.accumulate(st.u8[1], self.fid_stats[1], st.fid_rows)
 
     @torch.no_grad()
     def add(self, images: torch.Tensor) -> None:
@@ -169,10 +180,14 @@ class ReconstructionEvaluator:
         key = (B, H, W)
         st = self._steps.get(key)
         if st is None:
-            st = self._steps[key] = _Step(B, H, W, self.device, self.lpips is not None, self.save_dir is not None)
+            st = self._steps[key] = _Step(B, H, W, self.device, self.lpips is not None, self.save_dir is not None,
+                                          self.fid is not None)
         if st.copied is not None:
             torch.cuda.current_stream(self.device).wait_event(st.copied)  # the last batch's PNG copy has left st.u8
         st.x.copy_(images, non_blocking=True)
+        idx = png_indices(self.batches, self.batch_size, self.world, self.rank, B, self.total) if self.save_dir else []
+        if st.fid_rows is not None:
+            st.fid_rows.fill_(len(idx))
         if self.use_graph and st.graph is None and st.seen >= 1:
             torch.cuda.synchronize(self.device)
             g = torch.cuda.CUDAGraph()
@@ -189,7 +204,7 @@ class ReconstructionEvaluator:
         if st.lpips is not None:
             self._lpips.append(st.lpips.clone())
         if self.save_dir is not None:
-            self._save(st, png_indices(self.batches, self.batch_size, self.world, self.rank, B, self.total))
+            self._save(st, idx)
         self.batches += 1
 
     def _save(self, st: _Step, idx: List[int]) -> None:
@@ -218,15 +233,26 @@ class ReconstructionEvaluator:
         return out
 
     def result(self) -> Dict[str, object]:
-        """{'fid': None, 'psnr', 'lpips', 'ssim', 'num_samples'} aggregated as test_reconstruction_hf.py:415-466 (rFID is
-        computed by the command-line tool from the saved PNGs).  Waits for the device and the PNG writers."""
+        """{'fid', 'psnr', 'lpips', 'ssim', 'num_samples'} aggregated as test_reconstruction_hf.py:415-466.  'fid' is None
+        without an FID network (the command-line tool then computes rFID from the saved PNGs); with one, the ranks' S1,
+        S2 and n are summed and rank 0 gets the Fréchet distance (the other ranks None).  Waits for the device and the
+        PNG writers."""
         self.flush()
+        fid = None
+        if self.fid is not None:
+            from .fid import frechet_distance
+
+            if self.dist and self.world > 1:
+                for s in self.fid_stats:
+                    s.all_reduce()
+            if self.rank == 0 and self.fid_stats[0].count() >= 2:   # a covariance needs two images
+                fid = frechet_distance(*self.fid_stats[0].mu_sigma(), *self.fid_stats[1].mu_sigma())
         a = self.acc.cpu().tolist()
         n_img, n_batch = int(a[1]), int(a[4])
         psnr = a[0] / n_img if n_img else None
         ssim = a[2] / n_batch if n_batch else None
         lp = a[3] / n_batch if (n_batch and self.lpips is not None) else None
-        return {"fid": None, "psnr": rank_mean(psnr, self.world, self.device), "lpips": rank_mean(lp, self.world, self.device),
+        return {"fid": fid, "psnr": rank_mean(psnr, self.world, self.device), "lpips": rank_mean(lp, self.world, self.device),
                 "ssim": rank_mean(ssim, self.world, self.device), "num_samples": n_img * self.world}
 
     def flush(self) -> None:
@@ -274,6 +300,8 @@ def build_parser() -> argparse.ArgumentParser:
     ap.add_argument("--max_samples", type=int, default=None, help="evaluate only the first N images")
     ap.add_argument("--lpips_vgg", type=str, default=None, help="torchvision VGG16 checkpoint (features.* keys)")
     ap.add_argument("--lpips_lin", type=str, default=None, help="LPIPS lin weights (lin{0..4}.model.1.weight)")
+    ap.add_argument("--fid_weights", type=str, default=None,
+                    help="pytorch-fid's Inception weights (pt_inception-2015-12-05-6726825d.pth): rFID on the device")
     return ap
 
 
@@ -346,8 +374,18 @@ def run(args) -> Dict[str, object]:
         t = torch.tensor([int(skip)], device=device)
         dist.broadcast(t, src=0)
         skip = bool(t.item())
+    fid_net = None
+    if save and args.fid_weights:
+        from .fid import FIDInception
+
+        fid_net = FIDInception.from_file(args.fid_weights, device=device)
     if skip:
-        fid = compute_fid(ref_dir, save_dir, device) if main else None
+        if fid_net is not None:
+            from .fid import fid_from_paths
+
+            fid = fid_from_paths([ref_dir, save_dir], batch_size=50, num_workers=4, model=fid_net) if main else None
+        else:
+            fid = compute_fid(ref_dir, save_dir, device) if main else None
         if main:
             print(f"Found {total} reconstructed and reference images; skipped generation. rFID: {fid}")
         if args.use_ddp:
@@ -358,14 +396,14 @@ def run(args) -> Dict[str, object]:
                         pin_memory=True)
     lpips = LPIPSMetric.from_files(args.lpips_vgg, args.lpips_lin, device=device) if use_lpips else None
     ev = ReconstructionEvaluator(model, lpips=lpips, precision=args.precision, save_dir=args.output_path if save else None,
-                                 batch_size=args.batch_size, world=world, rank=rank, total=total)
+                                 batch_size=args.batch_size, world=world, rank=rank, total=total, fid=fid_net)
     for images, _ in loader:
         ev.add(images.to(device, non_blocking=True))
     res = ev.result()
     ev.close()
     if args.use_ddp:
         dist.barrier()
-    if save and main:
+    if save and main and fid_net is None:
         res["fid"] = compute_fid(ref_dir, save_dir, device)
     if main:
         print("Results:")
