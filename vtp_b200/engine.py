@@ -271,55 +271,55 @@ class DropPlan:
         return idx, scale
 
 
-def _block_drop(W: TowerW, bw: BlockW, x: torch.Tensor, B: int, T: int, rope, drop: DropPlan, t: Optional[dict]):
-    """One block of the fp32-stream trunk under batch-subset stochastic depth, bf16 (autocast) mode
-    (layers/block.py:201-233 / :238-289): gather the kept images, run the sub-layer on them, add the bf16 residual back
-    into a copy of the stream with alpha = residual_scale_factor."""
+def attention_sublayer(W: TowerW, bw: BlockW, x: torch.Tensor, n: int, T: int, mode: str, out: torch.Tensor,
+                       resid: Optional[torch.Tensor], tape: Optional[dict], *, rope, causal: bool) -> None:
+    """out = proj(attn(rope(qkv(norm1 x)))) (+ resid) on the n images of x [n*T, D] (layers/block.py:293,
+    attention.py:91-126).  A tape dict is filled with what the backward reads: x, rstd / mean, h, qkv, o, lse."""
     dev, D, H = x.device, W.D, W.heads
-    mode = "bf16"
-    # ---- attention sub-layer on subset 1
-    idx1, a1 = drop.next(B, dev)
-    n1 = idx1.numel()
-    M1 = n1 * T
-    xs1 = _e((M1, D), F32, dev)
-    lib.gather_images(x, xs1, idx1, T, D)
-    nt = {} if t is not None else None
-    h = norm(xs1, M1, D, bw.n1_w, bw.n1_b, W.eps, mode, want="op", tape=nt)
-    qkv = _e((M1, 3 * D), BF, dev)
-    linear(h, bw.qkv, qkv, M1, mode)
-    if rope is not None:
-        lib.rope_fwd(qkv, rope[0], rope[1], M1, T, W.prefix, D)
-    o = _e((M1, D), BF, dev)
-    lse = _e((n1, H, T), F32, dev) if t is not None else None
-    lib.attention_fwd(qkv, o, n1, T, H, prefix=W.prefix, lse=lse)
-    res1 = _e((M1, D), BF, dev)
-    linear(o, bw.proj, res1, M1, mode)
-    x_mid = x.clone()
-    lib.scatter_add_images(res1, x_mid, idx1, T, D, a1)
-    # ---- FFN sub-layer on subset 2 (drawn independently, block.py:219)
-    idx2, a2 = drop.next(B, dev)
-    n2 = idx2.numel()
-    M2 = n2 * T
-    xs2 = _e((M2, D), F32, dev)
-    lib.gather_images(x_mid, xs2, idx2, T, D)
-    nt2 = {} if t is not None else None
-    h2 = norm(xs2, M2, D, bw.n2_w, bw.n2_b, W.eps, mode, want="op", tape=nt2)
-    Hd = bw.hidden
-    pre = _e((M2, 2 * Hd), BF, dev)
-    hid = _e((M2, Hd), BF, dev)
-    if FUSED_SWIGLU:
-        linear(h2, bw.fc1, hid, M2, mode, act=lib.ACT_SWIGLU8, ldo=Hd, out2=pre)
+    M = n * T
+    act = BF if mode == "bf16" else F32
+    h = norm(x, M, D, bw.n1_w, bw.n1_b, W.eps, mode, want="op", tape=tape)
+    qkv = _e((M, 3 * D), act, dev)
+    if rope is not None and mode == "bf16" and SPLIT_EPILOGUES:
+        linear(h, bw.qkv, qkv, M, mode)                 # rounding to bf16 == q.to(bf16) of the reference
+        lib.rope_fwd(qkv, rope[0], rope[1], M, T, W.prefix, D)
+    elif rope is not None:
+        linear(h, bw.qkv, qkv, M, mode, act=lib.ACT_ROPE, rope=(rope[0], rope[1], T, W.prefix, 2 * D))
     else:
-        linear(h2, bw.fc1, pre, M2, mode)
-        lib.swiglu_fwd(pre, hid, M2, Hd)
-    res2 = _e((M2, D), BF, dev)
-    linear(hid, bw.fc2, res2, M2, mode)
-    x_out = x_mid.clone()
-    lib.scatter_add_images(res2, x_out, idx2, T, D, a2)
-    if t is not None:
-        t.update(drop1=(idx1, a1, xs1), drop2=(idx2, a2, xs2), h1=h, n1=nt, qkv=qkv, o=o, lse=lse, h2=h2, n2=nt2, pre=pre,
-                 hid=hid)
-    return x_out
+        linear(h, bw.qkv, qkv, M, mode)
+    o = _e((M, D), act, dev)
+    lse = _e((n, H, T), F32, dev) if tape is not None else None
+    if mode == "bf16":
+        lib.attention_fwd(qkv, o, n, T, H, prefix=W.prefix, causal=causal, lse=lse)
+    else:
+        lib.attention_fwd_f32(qkv, o, n, T, H, causal=causal)
+    linear(operand(o, M, D, mode), bw.proj, out, M, mode, resid=resid)
+    if tape is not None:
+        tape.update(x=x, h=h, qkv=qkv, o=o, lse=lse)
+
+
+def ffn_sublayer(W: TowerW, bw: BlockW, x: torch.Tensor, n: int, T: int, mode: str, out: torch.Tensor,
+                 resid: Optional[torch.Tensor], tape: Optional[dict]) -> None:
+    """out = w3(silu(w1 h) * w2 h)  /  c_proj(gelu(c_fc h)),  h = norm2 x  (+ resid) on the n images of x [n*T, D]
+    (layers/block.py:294).  A tape dict is filled with what the backward reads: x, rstd / mean, h, pre, hid."""
+    dev, D, Hd = x.device, W.D, bw.hidden
+    M = n * T
+    act = BF if mode == "bf16" else F32
+    h = norm(x, M, D, bw.n2_w, bw.n2_b, W.eps, mode, want="op", tape=tape)
+    hid = _e((M, Hd), act, dev)
+    if W.ffn == "swiglu" and mode == "bf16" and SPLIT_EPILOGUES and not FUSED_SWIGLU:
+        pre = _e((M, 2 * Hd), BF, dev)
+        linear(h, bw.fc1, pre, M, mode)
+        lib.swiglu_fwd(pre, hid, M, Hd)
+    elif W.ffn == "swiglu":
+        pre = _e((M, 2 * Hd), BF, dev) if tape is not None else None
+        linear(h, bw.fc1, hid, M, mode, act=lib.ACT_SWIGLU8, ldo=Hd, out2=pre)
+    else:
+        pre = _e((M, Hd), BF, dev) if tape is not None else None
+        linear(h, bw.fc1, hid, M, mode, act=lib.ACT_GELU, out2=pre)
+    linear(operand(hid, M, Hd, mode), bw.fc2, out, M, mode, resid=resid)
+    if tape is not None:
+        tape.update(x=x, h=h, pre=pre, hid=hid)
 
 
 def tower_blocks(W: TowerW, x: torch.Tensor, B: int, T: int, rope, mode: str, *, causal: bool = False,
@@ -327,73 +327,45 @@ def tower_blocks(W: TowerW, x: torch.Tensor, B: int, T: int, rope, mode: str, *,
                  drop: Optional[DropPlan] = None, hook: Optional[Callable[[int, torch.Tensor], None]] = None) -> torch.Tensor:
     """The block loop (encoders/vision_transformer.py:228-233, decoders/pixel_decoder.py:147-148,
     encoders/text_transformer.py:100-104): x [B*T, D] residual stream (fp32, or bf16 for the autocast decoder).
-    Inference updates x in place; with a tape every sub-layer writes a fresh stream buffer and saves what backward
-    needs.  `taps` {block index: None} is filled with copies of the stream after those blocks; `hook(li, x)` is called
-    after every block with the stream itself (read it before returning: inference overwrites it in place)."""
-    dev = x.device
-    M, D, H = B * T, W.D, W.heads
-    act = BF if mode == "bf16" else F32
-    if drop is not None and drop.ratio > 0.0:
-        if mode != "bf16" or W.stream_bf16 or W.ffn != "swiglu" or causal:
-            raise NotImplementedError("batch-subset stochastic depth is implemented for the vision trunk in bf16 mode "
-                                      "(the only tower the reference applies drop_ratio to: vtp.py:275-293,452-463,487-500)")
-        for li, bw in enumerate(W.blocks):
-            t = {} if tape is not None else None
-            x = _block_drop(W, bw, x, B, T, rope, drop, t)
-            if tape is not None:
-                tape.append(t)
-            if taps is not None and li in taps:
-                taps[li] = x.clone()
-            if hook is not None:
-                hook(li, x)
-        return x
+    Inference updates x in place; with a tape every sub-layer writes a fresh stream buffer and every block appends
+    {"attn": entry, "ffn": entry}, each entry holding what that sub-layer's backward reads plus its `subset`
+    ((idx, alpha) under stochastic depth, else None).  `taps` {block index: None} is filled with copies of the stream
+    after those blocks; `hook(li, x)` is called after every block with the stream itself (read it before returning:
+    inference overwrites it in place)."""
+    dev, D = x.device, W.D
+    on_subsets = drop is not None and drop.ratio > 0.0
+    if on_subsets and (mode != "bf16" or W.stream_bf16 or W.ffn != "swiglu" or causal):
+        raise NotImplementedError("batch-subset stochastic depth is implemented for the vision trunk in bf16 mode "
+                                  "(the only tower the reference applies drop_ratio to: vtp.py:275-293,452-463,487-500)")
+
+    def run(sublayer, bw: BlockW, x: torch.Tensor, e: Optional[dict], **kw) -> torch.Tensor:
+        """One sub-layer: on the whole stream with the residual added in its last GEMM's epilogue, or (stochastic
+        depth, layers/block.py:201-233) on a fresh random subset of the images, gathered, whose bf16 output is added
+        back into a copy of the stream with alpha = residual_scale_factor."""
+        subset = None
+        if not on_subsets:
+            out = x if e is None else torch.empty_like(x)
+            sublayer(W, bw, x, B, T, mode, out, x, e, **kw)
+        else:
+            idx, alpha = drop.next(B, dev)
+            n = idx.numel()
+            xs = _e((n * T, D), F32, dev)
+            lib.gather_images(x, xs, idx, T, D)
+            res = _e((n * T, D), BF, dev)
+            sublayer(W, bw, xs, n, T, mode, res, None, e, **kw)
+            out = x.clone()
+            lib.scatter_add_images(res, out, idx, T, D, alpha)
+            subset = (idx, alpha)
+        if e is not None:
+            e["subset"] = subset
+        return out
+
     for li, bw in enumerate(W.blocks):
-        t = {} if tape is not None else None
-        # ---- attention sub-layer: x + proj(attn(rope(qkv(norm1 x))))      layers/block.py:293, attention.py:91-126
-        nt = {} if t is not None else None
-        h = norm(x, M, D, bw.n1_w, bw.n1_b, W.eps, mode, want="op", tape=nt)
-        qkv = _e((M, 3 * D), act, dev)
-        if rope is not None and mode == "bf16" and SPLIT_EPILOGUES:
-            linear(h, bw.qkv, qkv, M, mode)                 # rounding to bf16 == q.to(bf16) of the reference
-            lib.rope_fwd(qkv, rope[0], rope[1], M, T, W.prefix, D)
-        elif rope is not None:
-            linear(h, bw.qkv, qkv, M, mode, act=lib.ACT_ROPE, rope=(rope[0], rope[1], T, W.prefix, 2 * D))
-        else:
-            linear(h, bw.qkv, qkv, M, mode)
-        o = _e((M, D), act, dev)
-        lse = _e((B, H, T), F32, dev) if t is not None else None
-        if mode == "bf16":
-            lib.attention_fwd(qkv, o, B, T, H, prefix=W.prefix, causal=causal, lse=lse)
-        else:
-            lib.attention_fwd_f32(qkv, o, B, T, H, causal=causal)
-        x_mid = x if t is None else torch.empty_like(x)
-        linear(operand(o, M, D, mode), bw.proj, x_mid, M, mode, resid=x)
-        if t is not None:
-            t.update(x_in=x, h1=h, n1=nt, qkv=qkv, o=o, lse=lse)
-        # ---- FFN sub-layer: x + w3(silu(w1 x) * w2 x)   /   x + c_proj(gelu(c_fc x))       layers/block.py:294
-        nt2 = {} if t is not None else None
-        h2 = norm(x_mid, M, D, bw.n2_w, bw.n2_b, W.eps, mode, want="op", tape=nt2)
-        Hd = bw.hidden
-        hid = _e((M, Hd), act, dev)
-        pre = None
-        if W.ffn == "swiglu" and mode == "bf16" and SPLIT_EPILOGUES and not FUSED_SWIGLU:
-            pre = _e((M, 2 * Hd), BF, dev)
-            linear(h2, bw.fc1, pre, M, mode)
-            lib.swiglu_fwd(pre, hid, M, Hd)
-            if t is None:
-                pre = None
-        elif W.ffn == "swiglu":
-            pre = _e((M, 2 * Hd), BF, dev) if t is not None else None
-            linear(h2, bw.fc1, hid, M, mode, act=lib.ACT_SWIGLU8, ldo=Hd, out2=pre)
-        else:
-            pre = _e((M, Hd), BF, dev) if t is not None else None
-            linear(h2, bw.fc1, hid, M, mode, act=lib.ACT_GELU, out2=pre)
-        x_out = x_mid if t is None else torch.empty_like(x)
-        linear(operand(hid, M, Hd, mode), bw.fc2, x_out, M, mode, resid=x_mid)
-        if t is not None:
-            t.update(x_mid=x_mid, h2=h2, n2=nt2, pre=pre, hid=hid)
-            tape.append(t)
-        x = x_out
+        ta, tf = ({}, {}) if tape is not None else (None, None)
+        x = run(attention_sublayer, bw, x, ta, rope=rope, causal=causal)
+        x = run(ffn_sublayer, bw, x, tf)
+        if tape is not None:
+            tape.append({"attn": ta, "ffn": tf})
         if taps is not None and li in taps:
             taps[li] = x.clone()
         if hook is not None:

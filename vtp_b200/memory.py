@@ -1,9 +1,12 @@
 """HBM budget of the 3-objective training step (what `VTPTrainer` keeps resident), used to size the per-pass image
 groups (`TrainConfig.ssl_chunk / rec_chunk`) for the 80 GB of an H100.
 
-The step saves, per token and per block, exactly what `engine.tower_blocks(..., tape=...)` appends:
-    x_in, x_mid (residual stream: fp32 in the trunk / text tower, bf16 in the autocast decoder), h1, h2, o (bf16 [D]),
-    qkv (bf16 [3D]), pre (bf16 [2·Hs] SwiGLU / [Hd] GELU), hid (bf16 [Hs] / [Hd]), lse + rstd (a few floats)
+The step saves, per token and per block, exactly what `engine.tower_blocks(..., tape=...)` appends, one entry per
+sub-layer:
+    attn: x (its norm's input: the residual stream, fp32 in the trunk / text tower, bf16 in the autocast decoder),
+          h (bf16 [D]), qkv (bf16 [3D]), o (bf16 [D]), lse + rstd (a few floats)
+    ffn:  x (as above), h (bf16 [D]), pre (bf16 [2·Hs] SwiGLU / [Hd] GELU), hid (bf16 [Hs] / [Hd]), rstd
+(under stochastic depth x is the gathered fp32 rows of the kept images, so the bytes scale with the kept fraction)
 => 20·D + 6·Hs bytes (fp32 stream, SwiGLU),  16·D + 6·Hs (bf16 stream),  20·D + 4·Hd (GELU MLP): `block_tape_bytes`.
 The three objectives run one after the other, so the peak is the largest single objective plus the persistent state.
 Calibration point (torch.cuda.max_memory_allocated on an H100, graph-captured step): VTP-Small, 256 images/GPU,

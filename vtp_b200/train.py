@@ -151,46 +151,75 @@ def attention_backward(t: dict, do: torch.Tensor, dqkv: torch.Tensor, B: int, T:
         lib.attention_bwd(t["qkv"], t["o"], do, t["lse"], dqkv, B, T, H, prefix=prefix, causal=causal, rope=rope)
 
 
+def attention_sublayer_backward(W: TowerW, bw: BlockW, gw: BlockW, e: dict, gb: torch.Tensor, dh: torch.Tensor, n: int,
+                                T: int, *, rope, causal: bool) -> None:
+    """Reverse of engine.attention_sublayer from its tape entry e: gb (bf16 dL/d(proj output) [n*T, D]) -> dh
+    (dL/d(norm1 output)); accumulates the proj and qkv weight gradients and the qkv bias gradient."""
+    M, D = n * T, W.D
+    do = _e((M, D), BF, gb.device)
+    dgrad(gb, bw.proj.w, do, M)
+    wgrad(gb, e["o"], gw.proj.w, M)
+    dqkv = _e((M, 3 * D), BF, gb.device)
+    attention_backward(e, do, dqkv, n, T, W.heads, W.prefix, causal, rope)
+    lib.cast_colsum(dqkv, None, gw.qkv.b, M, 3 * D)
+    dgrad(dqkv, bw.qkv.w, dh, M)
+    wgrad(dqkv, e["h"], gw.qkv.w, M)
+
+
+def ffn_sublayer_backward(W: TowerW, bw: BlockW, gw: BlockW, e: dict, gb: torch.Tensor, dh: torch.Tensor, n: int,
+                          T: int) -> None:
+    """Reverse of engine.ffn_sublayer from its tape entry e: gb (bf16 dL/d(fc2 output) [n*T, D]) -> dh
+    (dL/d(norm2 output)); accumulates the fc2 and fc1 weight gradients and the fc1 bias gradient."""
+    M, Hd = n * T, bw.hidden
+    dhid = _e((M, Hd), BF, gb.device)
+    dgrad(gb, bw.fc2.w, dhid, M)
+    wgrad(gb, e["hid"], gw.fc2.w, M)
+    dpre = torch.empty_like(e["pre"])
+    gate_bwd = lib.swiglu_bwd if W.ffn == "swiglu" else lib.gelu_bwd
+    gate_bwd(e["pre"], dhid, dpre, gw.fc1.b, M, Hd)
+    dgrad(dpre, bw.fc1.w, dh, M)
+    wgrad(dpre, e["h"], gw.fc1.w, M)
+
+
 def tower_blocks_backward(W: TowerW, G: TowerW, tape: list, g: torch.Tensor, B: int, T: int, rope, causal=False):
     """Reverse of engine.tower_blocks.  g fp32 [B*T, D]: in = dL/d(stream out), out = dL/d(stream in) (in place).
-    The bf16 copy of g (dY operand of the next sub-layer to differentiate) and its column sums (that sub-layer's bias
-    gradient) are by-products of the preceding norm_bwd; only the first sub-layer needs a stand-alone cast."""
-    dev = g.device
-    M, D, H = B * T, W.D, W.heads
-    nb = len(W.blocks)
-    if nb and "drop1" in tape[nb - 1]:
-        return _tower_blocks_backward_drop(W, G, tape, g, B, T, rope)
-    gb = _e((M, D), BF, dev)
-    lib.cast_colsum(g, gb, G.blocks[nb - 1].fc2.b, M, D)
-    for li in reversed(range(nb)):
+    Each sub-layer's body maps the bf16 dY operand gb of its last GEMM to dh; the edges around it follow its path.
+    Plain: g passes the residual unchanged, and gb with its column sums (that GEMM's bias gradient) is a by-product of
+    the norm_bwd of the sub-layer differentiated before it; only the first one needs a stand-alone cast.  Subset
+    (layers/block.py:201-233): d(residual) = alpha * g[idx] goes down the sub-layer, and what comes out of its norm
+    backward is scatter-added into g[idx]."""
+    dev, D = g.device, W.D
+    M = B * T
+    gb = dh = None
+    if tape[-1]["ffn"]["subset"] is None:
+        gb, dh = _e((M, D), BF, dev), _e((M, D), BF, dev)
+        lib.cast_colsum(g, gb, G.blocks[-1].fc2.b, M, D)
+
+    def run(body, bw, gw, e, norm_w, norm_gw, norm_gb, bias, next_bias, **kw):
+        """body with its path's edges.  bias: gradient of the sub-layer's last GEMM bias; next_bias: that of the
+        sub-layer differentiated next (None after the first block's attention)."""
+        if e["subset"] is None:
+            body(W, bw, gw, e, gb, dh, B, T, **kw)
+            lib.norm_bwd(e["x"], e["rstd"], e["mean"], norm_w, dh, g, norm_gw, norm_gb, M, D,
+                         gb_out=None if next_bias is None else gb, g_colsum=next_bias)
+            return
+        idx, alpha = e["subset"]
+        n = idx.numel()
+        gs = _e((n * T, D), F32, dev)
+        lib.gather_images(g, gs, idx, T, D, alpha)
+        gbs = _e((n * T, D), BF, dev)
+        lib.cast_colsum(gs, gbs, bias, n * T, D)
+        dhs = _e((n * T, D), BF, dev)
+        body(W, bw, gw, e, gbs, dhs, n, T, **kw)
+        gs.zero_()
+        lib.norm_bwd(e["x"], e["rstd"], e["mean"], norm_w, dhs, gs, norm_gw, norm_gb, n * T, D)
+        lib.scatter_add_images(gs, g, idx, T, D, 1.0)
+
+    for li in reversed(range(len(W.blocks))):
         bw, gw, t = W.blocks[li], G.blocks[li], tape[li]
-        Hd = bw.hidden
-        # ---- FFN sub-layer (gb / fc2 bias gradient already produced)
-        dhid = _e((M, Hd), BF, dev)
-        dgrad(gb, bw.fc2.w, dhid, M)
-        wgrad(gb, t["hid"], gw.fc2.w, M)
-        dpre = torch.empty_like(t["pre"])
-        if W.ffn == "swiglu":
-            lib.swiglu_bwd(t["pre"], dhid, dpre, gw.fc1.b, M, Hd)
-        else:
-            lib.gelu_bwd(t["pre"], dhid, dpre, gw.fc1.b, M, Hd)
-        dh = _e((M, D), BF, dev)
-        dgrad(dpre, bw.fc1.w, dh, M)
-        wgrad(dpre, t["h2"], gw.fc1.w, M)
-        lib.norm_bwd(t["x_mid"], t["n2"]["rstd"], t["n2"]["mean"], bw.n2_w, dh, g, gw.n2_w, gw.n2_b, M, D,
-                     gb_out=gb, g_colsum=gw.proj.b)
-        # ---- attention sub-layer
-        do = _e((M, D), BF, dev)
-        dgrad(gb, bw.proj.w, do, M)
-        wgrad(gb, t["o"], gw.proj.w, M)
-        dqkv = _e((M, 3 * D), BF, dev)
-        attention_backward(t, do, dqkv, B, T, H, W.prefix, causal, rope)
-        lib.cast_colsum(dqkv, None, gw.qkv.b, M, 3 * D)
-        dgrad(dqkv, bw.qkv.w, dh, M)
-        wgrad(dqkv, t["h1"], gw.qkv.w, M)
-        nxt = G.blocks[li - 1].fc2.b if li > 0 else None
-        lib.norm_bwd(t["x_in"], t["n1"]["rstd"], t["n1"]["mean"], bw.n1_w, dh, g, gw.n1_w, gw.n1_b, M, D,
-                     gb_out=gb if li > 0 else None, g_colsum=nxt)
+        run(ffn_sublayer_backward, bw, gw, t["ffn"], bw.n2_w, gw.n2_w, gw.n2_b, gw.fc2.b, gw.proj.b)
+        run(attention_sublayer_backward, bw, gw, t["attn"], bw.n1_w, gw.n1_w, gw.n1_b, gw.proj.b,
+            G.blocks[li - 1].fc2.b if li > 0 else None, rope=rope, causal=causal)
         tape[li] = None  # free the saved activations of this block
     return g
 
@@ -219,57 +248,6 @@ def grad_buckets(offset: Dict[str, int], n: int) -> Dict[str, List[Tuple[int, in
         else:
             r.append((off, end))
     return out
-
-
-def _tower_blocks_backward_drop(W: TowerW, G: TowerW, tape: list, g: torch.Tensor, B: int, T: int, rope):
-    """Reverse of engine._block_drop (batch-subset stochastic depth, layers/block.py:201-233).  The residual stream
-    gradient g passes every block unchanged (identity path); each sub-layer adds, for its kept images only, the gradient
-    that flows through  alpha * sublayer(norm(x[idx])) :  d(residual) = alpha * g[idx]  goes down the sub-layer, what
-    comes out of its norm backward is scatter-added into g[idx]."""
-    dev, D, H = g.device, W.D, W.heads
-    for li in reversed(range(len(W.blocks))):
-        bw, gw, t = W.blocks[li], G.blocks[li], tape[li]
-        Hd = bw.hidden
-        # ---- FFN sub-layer
-        idx2, a2, xs2 = t["drop2"]
-        M2 = idx2.numel() * T
-        gs = _e((M2, D), F32, dev)
-        lib.gather_images(g, gs, idx2, T, D, a2)
-        gb = _e((M2, D), BF, dev)
-        lib.cast_colsum(gs, gb, gw.fc2.b, M2, D)
-        dhid = _e((M2, Hd), BF, dev)
-        dgrad(gb, bw.fc2.w, dhid, M2)
-        wgrad(gb, t["hid"], gw.fc2.w, M2)
-        dpre = torch.empty_like(t["pre"])
-        lib.swiglu_bwd(t["pre"], dhid, dpre, gw.fc1.b, M2, Hd)
-        dh = _e((M2, D), BF, dev)
-        dgrad(dpre, bw.fc1.w, dh, M2)
-        wgrad(dpre, t["h2"], gw.fc1.w, M2)
-        gsub = gs.zero_()
-        lib.norm_bwd(xs2, t["n2"]["rstd"], t["n2"]["mean"], bw.n2_w, dh, gsub, gw.n2_w, gw.n2_b, M2, D)
-        lib.scatter_add_images(gsub, g, idx2, T, D, 1.0)
-        # ---- attention sub-layer
-        idx1, a1, xs1 = t["drop1"]
-        n1 = idx1.numel()
-        M1 = n1 * T
-        gs = _e((M1, D), F32, dev)
-        lib.gather_images(g, gs, idx1, T, D, a1)
-        gb = _e((M1, D), BF, dev)
-        lib.cast_colsum(gs, gb, gw.proj.b, M1, D)
-        do = _e((M1, D), BF, dev)
-        dgrad(gb, bw.proj.w, do, M1)
-        wgrad(gb, t["o"], gw.proj.w, M1)
-        dqkv = _e((M1, 3 * D), BF, dev)
-        attention_backward(t, do, dqkv, n1, T, H, W.prefix, False, rope)
-        lib.cast_colsum(dqkv, None, gw.qkv.b, M1, 3 * D)
-        dh = _e((M1, D), BF, dev)
-        dgrad(dqkv, bw.qkv.w, dh, M1)
-        wgrad(dqkv, t["h1"], gw.qkv.w, M1)
-        gsub = gs.zero_()
-        lib.norm_bwd(xs1, t["n1"]["rstd"], t["n1"]["mean"], bw.n1_w, dh, gsub, gw.n1_w, gw.n1_b, M1, D)
-        lib.scatter_add_images(gsub, g, idx1, T, D, 1.0)
-        tape[li] = None
-    return g
 
 
 # ------------------------------------------------------------------------------------------------------ trainer
