@@ -65,21 +65,15 @@ def test_latent_statistics_formula():
     assert torch.allclose(st["std"].double(), z.std(dim=(0, 2, 3), keepdim=True), atol=1e-6)
 
 
-def test_gradient_buckets_partition_the_flat_buffer():
+def test_gradient_buckets_partition_the_table_store():
     """train.grad_buckets: the per-tower all-reduce ranges cover [0, n) exactly once, and every tensor lies inside the
     bucket of its tower (text + clip projection + logit scale | DINO head | pixel decoder | trunk)."""
-    from vtp_b200.train import ParamStore, _vit_specs, grad_buckets
+    from vtp_b200.params import table
+    from vtp_b200.train import ParamStore, grad_buckets
 
     st = ParamStore("cpu")
-    st.add("trunk.patch.w", (128, 768), True, True); st.add("trunk.cls", (128,), False, True)
-    _vit_specs(st, "trunk.", 128, 2, 344, False, True, 688)
-    st.add("visual_proj.w", (128, 128), True, True)
-    st.add("head.mlp0.w", (256, 128), True, True); st.add("head.last_g", (512,), False, True)
-    st.add("decoder.proj_in.w", (128, 64), True)
-    _vit_specs(st, "decoder.", 128, 2, 344, True, False, 688)
-    st.add("text.tok_emb", (1000, 128), True); st.add("text.pos", (77, 128), False)
-    _vit_specs(st, "text.", 128, 2, 512, True, False, 512)
-    st.add("logit_scale", (1,), False)
+    for e in table(preset("tiny"), (512, 256, 64)):
+        st.add(e.name, e.shape, e.decay, e.teacher)
     st.finalize()
     b = grad_buckets(st.offset, st.n)
     ranges = sorted(r for rs in b.values() for r in rs)

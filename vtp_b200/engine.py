@@ -112,85 +112,6 @@ class TowerW:
         return self._rope[key]
 
 
-def _f(t):
-    return t.detach().to(F32).contiguous()
-
-
-def pack_vit_blocks(sd: Dict[str, torch.Tensor], pre: str, depth: int, mode: str, ln: bool) -> List[BlockW]:
-    blocks = []
-    for i in range(depth):
-        p = f"{pre}blocks.{i}."
-        w1, w2 = sd[p + "mlp.w1.weight"], sd[p + "mlp.w2.weight"]
-        Hs = w1.shape[0]
-        blocks.append(BlockW(
-            n1_w=_f(sd[p + "norm1.weight"]), n1_b=_f(sd[p + "norm1.bias"]) if ln else None,
-            qkv=pack_lin(sd[p + "attn.qkv.weight"], sd.get(p + "attn.qkv.bias"), mode),
-            proj=pack_lin(sd[p + "attn.proj.weight"], sd.get(p + "attn.proj.bias"), mode),
-            n2_w=_f(sd[p + "norm2.weight"]), n2_b=_f(sd[p + "norm2.bias"]) if ln else None,
-            fc1=pack_lin(interleave8(w1, w2), interleave8(sd[p + "mlp.w1.bias"], sd[p + "mlp.w2.bias"]), mode),
-            fc2=pack_lin(sd[p + "mlp.w3.weight"], sd.get(p + "mlp.w3.bias"), mode),
-            hidden=Hs))
-    return blocks
-
-
-def pack_trunk(sd, cfg, mode: str, pre: str = "trunk.") -> TowerW:
-    """encoders/vision_transformer.py:58-187 + vision_transformer_bottleneck.py:11-46 parameters."""
-    ln = cfg.vision_norm_layer != "rmsnorm"
-    eps = {"rmsnorm": 1e-5, "layernorm": 1e-6, "layernormbf16": 1e-5}[cfg.vision_norm_layer]
-    W = TowerW(D=cfg.vision_embed_dim, heads=cfg.vision_num_heads, norm="ln" if ln else "rms", eps=eps,
-               stream_bf16=False, prefix=1, ffn="swiglu")
-    W.blocks = pack_vit_blocks(sd, pre, cfg.vision_depth, mode, ln)
-    W.norm_w = _f(sd[pre + "norm.weight"])
-    W.norm_b = _f(sd[pre + "norm.bias"]) if ln else None
-    W.periods = sd[pre + "rope_embed.periods"].detach().cpu()
-    pw = sd[pre + "patch_embed.proj.weight"]
-    W.extra["patch"] = pack_lin(pw.flatten(1), sd[pre + "patch_embed.proj.bias"], mode)
-    W.extra["patch_size"] = pw.shape[-1]
-    cls = _f(sd[pre + "cls_token"]).reshape(-1) + 0 * _f(sd[pre + "mask_token"]).reshape(-1)
-    W.extra["cls"] = cls.contiguous()
-    mt = _f(sd[pre + "mask_token"]).reshape(-1)
-    W.extra["mask_token"] = (mt.to(BF).to(F32) if mode == "bf16" else mt).contiguous()
-    if (pre + "feature_bottleneck.weight") in sd:
-        W.extra["bneck"] = pack_lin(sd[pre + "feature_bottleneck.weight"], None, mode)
-    return W
-
-
-def pack_decoder(sd, cfg, mode: str, pre: str = "pixel_decoder.") -> TowerW:
-    """decoders/pixel_decoder.py:15-132 parameters."""
-    ln = cfg.decoder_norm_layer != "rmsnorm"
-    eps = {"rmsnorm": 1e-5, "layernorm": 1e-6, "layernormbf16": 1e-5}[cfg.decoder_norm_layer]
-    W = TowerW(D=cfg.decoder_embed_dim, heads=cfg.decoder_num_heads, norm="ln" if ln else "rms", eps=eps,
-               stream_bf16=(mode == "bf16"), prefix=0, ffn="swiglu")
-    W.blocks = pack_vit_blocks(sd, pre, cfg.decoder_depth, mode, ln)
-    W.norm_w = _f(sd[pre + "norm.weight"])
-    W.norm_b = _f(sd[pre + "norm.bias"]) if ln else None
-    W.periods = sd[pre + "rope_embed.periods"].detach().cpu()
-    W.extra["proj_in"] = pack_lin(sd[pre + "proj_in.weight"].flatten(1), sd.get(pre + "proj_in.bias"), mode)
-    W.extra["proj_out"] = pack_lin(sd[pre + "proj_out.weight"].flatten(1), sd.get(pre + "proj_out.bias"), mode)
-    return W
-
-
-def pack_text(sd, cfg, mode: str, pre: str = "text_transformer.") -> TowerW:
-    """encoders/text_transformer.py:231-332 + layers/block.py:370-427 parameters."""
-    W = TowerW(D=cfg.text_embed_dim, heads=cfg.text_num_heads, norm="ln", eps=1e-5, stream_bf16=False, prefix=0,
-               ffn="gelu")
-    for i in range(cfg.text_depth):
-        p = f"{pre}resblocks.{i}."
-        W.blocks.append(BlockW(
-            n1_w=_f(sd[p + "ln_1.weight"]), n1_b=_f(sd[p + "ln_1.bias"]),
-            qkv=pack_lin(sd[p + "attn.in_proj_weight"], sd[p + "attn.in_proj_bias"], mode),
-            proj=pack_lin(sd[p + "attn.out_proj.weight"], sd[p + "attn.out_proj.bias"], mode),
-            n2_w=_f(sd[p + "ln_2.weight"]), n2_b=_f(sd[p + "ln_2.bias"]),
-            fc1=pack_lin(sd[p + "mlp.c_fc.weight"], sd[p + "mlp.c_fc.bias"], mode),
-            fc2=pack_lin(sd[p + "mlp.c_proj.weight"], sd[p + "mlp.c_proj.bias"], mode),
-            hidden=sd[p + "mlp.c_fc.weight"].shape[0]))
-    W.norm_w, W.norm_b = _f(sd["ln_final.weight"]), _f(sd["ln_final.bias"])
-    W.extra["tok_emb"] = _f(sd["token_embedding.weight"])
-    W.extra["pos"] = _f(sd["positional_embedding"])
-    W.extra["proj"] = pack_lin(sd["text_projection"].t(), None, mode)  # x @ P  ==  linear(x, Pᵀ)
-    return W
-
-
 # ------------------------------------------------------------------------------------------------------ primitives
 def operand(x: torch.Tensor, M: int, K: int, mode: str) -> torch.Tensor:
     """GEMM A operand of an activation: bf16 mode -> x itself (bf16); fp32 mode -> bf16x3 split [M, 3K]."""

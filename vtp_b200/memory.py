@@ -14,16 +14,13 @@ K = 65 536 -> 42.7 GiB peak.
 """
 from __future__ import annotations
 
+import math
 from typing import Dict, Tuple
 
 from .config import VTPConfig
+from .params import Geometry, geometry, table
 
 GIB = float(2 ** 30)
-
-
-def _swiglu_hidden(dim: int, ratio: float, align: int = 8) -> int:
-    d = int(int(dim * ratio) * 2 / 3)
-    return d + (-d % align)
 
 
 def block_tape_bytes(D: int, hidden: int, ffn: str, stream_bf16: bool, heads: int) -> int:
@@ -33,26 +30,14 @@ def block_tape_bytes(D: int, hidden: int, ffn: str, stream_bf16: bool, heads: in
     return 2 * s * D + 3 * 2 * D + 2 * 3 * D + pre + 2 * hidden + 4 * heads + 8
 
 
-def tower_tape_bytes(tokens: int, D: int, depth: int, hidden: int, ffn: str, stream_bf16: bool, heads: int) -> int:
-    return tokens * depth * block_tape_bytes(D, hidden, ffn, stream_bf16, heads)
+def tower_tape_bytes(tokens: int, g: Geometry) -> int:
+    return tokens * g.depth * block_tape_bytes(g.D, g.hidden, g.ffn, g.stream_bf16, g.heads)
 
 
 def param_count(cfg: VTPConfig, head_out_dim: int = 65536, head_hidden: int = 2048, head_bottleneck: int = 256) -> Dict[str, int]:
-    D, Dd, Dt = cfg.vision_embed_dim, cfg.decoder_embed_dim, cfg.text_embed_dim
-    hs, hsd, ht = _swiglu_hidden(D, cfg.vision_mlp_ratio), _swiglu_hidden(Dd, 4.0), int(Dt * cfg.text_mlp_ratio)
-    ps, bn = cfg.vision_patch_size, cfg.vision_feature_bottleneck or D
-
-    def vit(dim, depth, hidden, swiglu):
-        per = 4 * dim * dim + 4 * dim + (3 * dim * hidden + 2 * hidden + dim if swiglu else 2 * dim * hidden + hidden + dim) + 4 * dim
-        return depth * per + 2 * dim
-
-    trunk = vit(D, cfg.vision_depth, hs, True) + D * 3 * ps * ps + 3 * D + bn * D + Dt * D
-    head = D * head_hidden + head_hidden ** 2 + head_hidden * head_bottleneck + 2 * head_hidden + head_bottleneck + \
-        head_out_dim * (head_bottleneck + 1)
-    dec = vit(Dd, cfg.decoder_depth, hsd, True) + Dd * bn + Dd + 768 * Dd + 768
-    text = vit(Dt, cfg.text_depth, ht, False) + cfg.text_vocab_size * Dt + cfg.text_context_length * Dt + Dt * Dt
-    return {"trunk": trunk, "head": head, "decoder": dec, "text": text, "teacher": trunk + head,
-            "total": trunk + head + dec + text}
+    """Parameters of the training step: all of them, and those the EMA teacher keeps a copy of."""
+    sizes = [(math.prod(e.shape), e.teacher) for e in table(cfg, (head_out_dim, head_hidden, head_bottleneck))]
+    return {"total": sum(n for n, _ in sizes), "teacher": sum(n for n, t in sizes if t)}
 
 
 def train_step_bytes(cfg: VTPConfig, B: int, *, image: int = 256, local: int = 96, n_local: int = 8,
@@ -60,9 +45,8 @@ def train_step_bytes(cfg: VTPConfig, B: int, *, image: int = 256, local: int = 9
                      mask_ratio: float = 0.3, mask_prob: float = 0.5, ssl_chunk: int = 0, rec_chunk: int = 0,
                      lpips: bool = True, lpips_chunk: int = 32) -> Dict[str, float]:
     """Estimated resident bytes: persistent state + the peak of each objective (they run sequentially)."""
-    D, Dd, Dt = cfg.vision_embed_dim, cfg.decoder_embed_dim, cfg.text_embed_dim
-    H, Hd_, Ht = cfg.vision_num_heads, cfg.decoder_num_heads, cfg.text_num_heads
-    hs, hsd, ht = _swiglu_hidden(D, cfg.vision_mlp_ratio), _swiglu_hidden(Dd, 4.0), int(Dt * cfg.text_mlp_ratio)
+    gv, gd, gt = (geometry(cfg, tower) for tower in ("trunk", "decoder", "text"))
+    D, Dd, hs, hsd = gv.D, gd.D, gv.hidden, gd.hidden
     ps = cfg.vision_patch_size
     HW, HWl = (image // ps) ** 2, (local // ps) ** 2
     T, Tl = HW + 1, HWl + 1
@@ -72,14 +56,13 @@ def train_step_bytes(cfg: VTPConfig, B: int, *, image: int = 256, local: int = 9
     inputs = B * (3 * image * image * 4 * (1 + 2 + 1) + n_local * 3 * local * local * 4)
 
     def trunk(tokens):
-        return tower_tape_bytes(tokens, D, cfg.vision_depth, hs, "swiglu", False, H) + tokens * (4 * D + 2 * 3 * ps * ps)
+        return tower_tape_bytes(tokens, gv) + tokens * (4 * D + 2 * 3 * ps * ps)
 
     # transient working set of one backward sub-layer (dh, dhid, dpre, dqkv, do, g, gb ...) on the largest token group
     def transient(tokens, dim, hidden):
         return tokens * (4 * dim * 2 + 2 * dim * 2 + 2 * hidden * 3 * 2 + 2 * 3 * dim)
 
-    clip = trunk(B * T) + tower_tape_bytes(B * cfg.text_context_length, Dt, cfg.text_depth, ht, "gelu", False, Ht) + \
-        transient(B * T, D, hs)
+    clip = trunk(B * T) + tower_tape_bytes(B * cfg.text_context_length, gt) + transient(B * T, D, hs)
     bs = ssl_chunk if 0 < ssl_chunk < B else B
     n_m = int(round(2 * bs * mask_prob * mask_ratio * HW))
     rows_s, rows_t = n_local * bs + 2 * bs + n_m, 2 * bs + n_m
@@ -88,8 +71,7 @@ def train_step_bytes(cfg: VTPConfig, B: int, *, image: int = 256, local: int = 9
     br = rec_chunk if 0 < rec_chunk < B else B
     vgg_per_img = 2 * (64 * 2 * image ** 2 + 128 * 2 * (image // 2) ** 2 + 256 * 3 * (image // 4) ** 2 +
                        512 * 3 * (image // 8) ** 2 + 512 * 3 * (image // 16) ** 2)
-    rec = trunk(br * T) + tower_tape_bytes(br * HW, Dd, cfg.decoder_depth, hsd, "swiglu", True, Hd_) + \
-        br * 3 * image * image * (2 + 4 + 2) + transient(br * HW, Dd, hsd) + \
+    rec = trunk(br * T) + tower_tape_bytes(br * HW, gd) + br * 3 * image * image * (2 + 4 + 2) + transient(br * HW, Dd, hsd) + \
         (2 * 2 * min(lpips_chunk, br) * vgg_per_img if lpips else 0)
     peak = persistent + inputs + max(clip, ssl, rec)
     return {"persistent": persistent, "inputs": inputs, "clip": clip, "ssl": ssl, "rec": rec, "peak": peak,

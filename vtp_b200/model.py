@@ -28,17 +28,11 @@ from torch import nn
 
 from . import engine as E
 from . import lib
+from . import params as P
 from .config import VTPConfig
 from .rope import rope_periods
 
 BF = torch.bfloat16
-
-
-def _swiglu_hidden(dim: int, ratio: float, ffn_layer: str) -> int:
-    """layers/block.py:176 + layers/ffn.py:71-72 (+ align variants encoders/vision_transformer.py:22-28)."""
-    align = {"swiglu": 8, "swiglu32": 32, "swiglu64": 64, "swiglu128": 128}[ffn_layer]
-    d = int(int(dim * ratio) * 2 / 3)
-    return d + (-d % align)
 
 
 def check_head_dims(c: VTPConfig) -> None:
@@ -176,7 +170,7 @@ class VTPModel(VTPPreTrainedModel):
         t.patch_embed.proj.bias = _param(D)
         t.rope_embed = _Holder()
         t.rope_embed.register_buffer("periods", rope_periods(D // c.vision_num_heads), persistent=True)
-        hs = _swiglu_hidden(D, c.vision_mlp_ratio, c.vision_ffn_layer)
+        hs = P.swiglu_hidden(D, c.vision_mlp_ratio, c.vision_ffn_layer)
         t.blocks = nn.ModuleList([_vit_block_holder(D, hs, ln) for _ in range(c.vision_depth)])
         t.norm = _norm_holder(D, ln)
         if c.vision_feature_bottleneck is not None and c.vision_feature_bottleneck != D:
@@ -198,7 +192,7 @@ class VTPModel(VTPPreTrainedModel):
             d.proj_in.bias = _param(Dd)
             d.rope_embed = _Holder()
             d.rope_embed.register_buffer("periods", rope_periods(Dd // c.decoder_num_heads), persistent=True)
-            hsd = _swiglu_hidden(Dd, 4.0, c.decoder_ffn_layer)
+            hsd = P.swiglu_hidden(Dd, 4.0, c.decoder_ffn_layer)
             d.blocks = nn.ModuleList([_vit_block_holder(Dd, hsd, lnd) for _ in range(c.decoder_depth)])
             d.norm = _norm_holder(Dd, lnd)
             d.proj_out = _Holder()
@@ -374,18 +368,8 @@ class VTPModel(VTPPreTrainedModel):
             raise lib.VtpError("VTPModel runs only on a CUDA (sm_90a) device; move the model with .cuda() — there is "
                                "no CPU path")
         lib.check(lib.load().vtp_check_device(), "vtp_check_device")
-        sd = {k: v for k, v in self.state_dict().items()}
         with torch.no_grad():
-            if tower == "trunk":
-                W = E.pack_trunk(sd, self.config, mode)
-                if self.visual_proj is not None:
-                    W.extra["visual_proj"] = E.pack_lin(sd["visual_proj.weight"], None, mode)
-            elif tower == "decoder":
-                W = E.pack_decoder(sd, self.config, mode)
-            elif tower == "text":
-                W = E.pack_text(sd, self.config, mode)
-            else:  # pragma: no cover
-                raise KeyError(tower)
+            W = P.pack_tower(self.state_dict(), self.config, tower, mode)
         self._packs[(tower, mode)] = (ver, W)
         return W
 

@@ -21,8 +21,10 @@ import torch
 
 from . import engine as E
 from . import lib
+from . import params as P
 from .config import VTPConfig
 from .engine import BF, F32, BlockW, Lin, TowerW, _e
+from .rope import rope_periods
 
 _ALIGN = 64  # elements; keeps every tensor 128B-aligned in the bf16 copy (TMA needs 16B)
 
@@ -84,44 +86,19 @@ class ParamStore:
             self.tpb.copy_(self.pb[:self.n_teacher])
 
 
-def _vit_specs(store: ParamStore, pre: str, D: int, depth: int, hidden: int, ln: bool, teacher: bool, ffn_out: int):
-    for i in range(depth):
-        p = f"{pre}blocks.{i}."
-        store.add(p + "n1_w", (D,), False, teacher)
-        if ln: store.add(p + "n1_b", (D,), False, teacher)
-        store.add(p + "qkv.w", (3 * D, D), True, teacher); store.add(p + "qkv.b", (3 * D,), False, teacher)
-        store.add(p + "proj.w", (D, D), True, teacher); store.add(p + "proj.b", (D,), False, teacher)
-        store.add(p + "n2_w", (D,), False, teacher)
-        if ln: store.add(p + "n2_b", (D,), False, teacher)
-        store.add(p + "fc1.w", (ffn_out, D), True, teacher); store.add(p + "fc1.b", (ffn_out,), False, teacher)
-        store.add(p + "fc2.w", (D, hidden), True, teacher); store.add(p + "fc2.b", (D,), False, teacher)
-    store.add(pre + "norm_w", (D,), False, teacher)
-    if ln: store.add(pre + "norm_b", (D,), False, teacher)
-
-
-def _tower_views(store: ParamStore, pre: str, tw: TowerW, depth: int, hidden: int, ln: bool, *, kind: str):
-    """kind: 'param' (bf16 weights + fp32 vectors), 'teacher', or 'grad' (fp32 gradient views)."""
-    if kind == "param":
-        wv, fv = store.bf16, store.f32
-    elif kind == "teacher":
-        wv, fv = store.tbf16, store.tf32
-    else:
-        wv, fv = store.grad, store.grad
-
+def store_tower(cfg: VTPConfig, names, tower: str, wv, fv) -> TowerW:
+    """One tower as views of the flat buffers: GEMM weights through wv(name), vectors and biases through fv(name);
+    `names` holds the store names.  The trunk also carries the bottleneck, the clip projection and the DINO head."""
     def lin(name):
         w = wv(name + ".w")
-        b = fv(name + ".b") if (name + ".b") in store.offset else None
-        return Lin(w, b, w.shape[0], w.shape[1])
+        return Lin(w, fv(name + ".b") if name + ".b" in names else None, w.shape[0], w.shape[1])
 
-    tw.blocks = []
-    for i in range(depth):
-        p = f"{pre}blocks.{i}."
-        tw.blocks.append(BlockW(n1_w=fv(p + "n1_w"), n1_b=fv(p + "n1_b") if ln else None, qkv=lin(p + "qkv"),
-                                proj=lin(p + "proj"), n2_w=fv(p + "n2_w"), n2_b=fv(p + "n2_b") if ln else None,
-                                fc1=lin(p + "fc1"), fc2=lin(p + "fc2"), hidden=hidden))
-    tw.norm_w = fv(pre + "norm_w")
-    tw.norm_b = fv(pre + "norm_b") if ln else None
-    return lin
+    W = P.assemble(cfg, tower, "bf16", fv, lin)
+    W.periods = rope_periods(64)
+    if tower == "trunk":
+        W.extra.update(bneck=lin("trunk.bneck"), visual_proj=lin("visual_proj"), mlp0=lin("head.mlp0"),
+                       mlp2=lin("head.mlp2"), mlp4=lin("head.mlp4"), last_v=fv("head.last_v"), last_g=fv("head.last_g"))
+    return W
 
 
 # ------------------------------------------------------------------------------------------------------ backward
@@ -303,38 +280,21 @@ class VTPTrainer:
         c = cfg
         if c.vision_norm_layer != "rmsnorm" or c.decoder_norm_layer not in ("layernorm", "layernormbf16"):
             raise NotImplementedError("trainer supports the reference defaults: rmsnorm trunk, layernorm decoder")
-        from .model import _swiglu_hidden, check_head_dims
+        from .model import check_head_dims
         if not (c.train_clip and c.train_reconstruction):
             raise NotImplementedError("the trainer runs all three objectives: train_clip and train_reconstruction must be on")
+        if not c.vision_bottleneck_ae_only:
+            raise NotImplementedError("the trainer projects the trunk's cls token, not its bottleneck features, for the "
+                                      "contrastive objective (vision_bottleneck_ae_only=True)")
         check_head_dims(c)
         self.D, self.Dd, self.Dt = c.vision_embed_dim, c.decoder_embed_dim, c.text_embed_dim
-        self.hs = _swiglu_hidden(self.D, c.vision_mlp_ratio, c.vision_ffn_layer)
-        self.hsd = _swiglu_hidden(self.Dd, 4.0, c.decoder_ffn_layer)
-        self.ht = int(self.Dt * c.text_mlp_ratio)
+        self.hs = P.geometry(c, "trunk").hidden
         self.bn = c.vision_feature_bottleneck
+        K, hb = self.tc.head_out_dim, self.tc.head_bottleneck
+        self.table = P.table(c, (K, self.tc.head_hidden, hb))
         st = ParamStore(self.device)
-        D, Dd, Dt, K = self.D, self.Dd, self.Dt, self.tc.head_out_dim
-        ps = c.vision_patch_size
-        # trunk (+ clip projection + DINO head): these have an EMA teacher (vtp.py:239-262)
-        st.add("trunk.patch.w", (D, 3 * ps * ps), True, True); st.add("trunk.patch.b", (D,), False, True)
-        st.add("trunk.cls", (D,), False, True); st.add("trunk.mask_token", (D,), False, True)
-        _vit_specs(st, "trunk.", D, c.vision_depth, self.hs, False, True, 2 * self.hs)
-        st.add("trunk.bneck.w", (self.bn, D), True, True)
-        st.add("visual_proj.w", (Dt, D), True, True)
-        hh, hb = self.tc.head_hidden, self.tc.head_bottleneck
-        st.add("head.mlp0.w", (hh, D), True, True); st.add("head.mlp0.b", (hh,), False, True)
-        st.add("head.mlp2.w", (hh, hh), True, True); st.add("head.mlp2.b", (hh,), False, True)
-        st.add("head.mlp4.w", (hb, hh), True, True); st.add("head.mlp4.b", (hb,), False, True)
-        st.add("head.last_v", (K, hb), True, True); st.add("head.last_g", (K,), False, True)
-        # decoder
-        st.add("decoder.proj_in.w", (Dd, self.bn), True); st.add("decoder.proj_in.b", (Dd,), False)
-        _vit_specs(st, "decoder.", Dd, c.decoder_depth, self.hsd, True, False, 2 * self.hsd)
-        st.add("decoder.proj_out.w", (3 * 256, Dd), True); st.add("decoder.proj_out.b", (3 * 256,), False)
-        # text
-        st.add("text.tok_emb", (c.text_vocab_size, Dt), True); st.add("text.pos", (c.text_context_length, Dt), False)
-        _vit_specs(st, "text.", Dt, c.text_depth, self.ht, True, False, self.ht)
-        st.add("text.proj.w", (Dt, Dt), True)
-        st.add("logit_scale", (1,), False)
+        for e in self.table:
+            st.add(e.name, e.shape, e.decay, e.teacher)
         st.finalize()
         self.store = st
         self._build_towers()
@@ -387,36 +347,11 @@ class VTPTrainer:
 
     # -------------------------------------------------------------- towers as views of the flat buffers
     def _build_towers(self):
-        c, st = self.cfg, self.store
-
-        def mk(pre, D, heads, depth, hidden, ln, norm, eps, stream_bf16, prefix, ffn, kind):
-            tw = TowerW(D=D, heads=heads, norm=norm, eps=eps, stream_bf16=stream_bf16, prefix=prefix, ffn=ffn)
-            lin = _tower_views(st, pre, tw, depth, hidden, ln, kind=kind)
-            from .rope import rope_periods
-            tw.periods = rope_periods(64)
-            return tw, lin
-
-        self.towers = {}
-        for kind in ("param", "teacher", "grad"):
-            tw, lin = mk("trunk.", self.D, c.vision_num_heads, c.vision_depth, self.hs, False, "rms", 1e-5, False, 1,
-                         "swiglu", kind)
-            fv = {"param": st.f32, "teacher": st.tf32, "grad": st.grad}[kind]
-            tw.extra.update(patch=lin("trunk.patch"), patch_size=c.vision_patch_size, cls=fv("trunk.cls"),
-                            mask_token=fv("trunk.mask_token"), bneck=lin("trunk.bneck"),
-                            visual_proj=lin("visual_proj"), mlp0=lin("head.mlp0"), mlp2=lin("head.mlp2"),
-                            mlp4=lin("head.mlp4"), last_v=fv("head.last_v"), last_g=fv("head.last_g"))
-            self.towers[("trunk", kind)] = tw
-        for kind in ("param", "grad"):
-            eps_d = 1e-6 if c.decoder_norm_layer == "layernorm" else 1e-5
-            tw, lin = mk("decoder.", self.Dd, c.decoder_num_heads, c.decoder_depth, self.hsd, True, "ln", eps_d, True, 0,
-                         "swiglu", kind)
-            tw.extra.update(proj_in=lin("decoder.proj_in"), proj_out=lin("decoder.proj_out"))
-            self.towers[("decoder", kind)] = tw
-            tw, lin = mk("text.", self.Dt, c.text_num_heads, c.text_depth, self.ht, True, "ln", 1e-5, False, 0, "gelu",
-                         kind)
-            fv = st.f32 if kind == "param" else st.grad
-            tw.extra.update(tok_emb=fv("text.tok_emb"), pos=fv("text.pos"), proj=lin("text.proj"))
-            self.towers[("text", kind)] = tw
+        st = self.store
+        views = {"param": (st.bf16, st.f32), "teacher": (st.tbf16, st.tf32), "grad": (st.grad, st.grad)}
+        self.towers = {(tower, kind): store_tower(self.cfg, st.offset, tower, *views[kind])
+                       for tower, kinds in (("trunk", ("param", "teacher", "grad")), ("decoder", ("param", "grad")),
+                                            ("text", ("param", "grad"))) for kind in kinds}
 
     # -------------------------------------------------------------- init / state-dict exchange
     @torch.no_grad()
@@ -443,105 +378,13 @@ class VTPTrainer:
     def import_state_dict(self, sd: Dict[str, torch.Tensor], head_sd: Optional[Dict[str, torch.Tensor]] = None):
         """Load a reference-format VTPModel state dict (+ optional DINOHead state dict with keys mlp.0.weight, ...,
         last_layer.weight_g / weight_v or the parametrizations.* spelling)."""
-        st = self.store
-        dev = self.device
-
-        def put(name, t):
-            st.f32(name).copy_(t.to(dev, F32).reshape(st.shape[name]))
-
-        def vit(pre_ref, pre, depth, ln, swiglu=True):
-            for i in range(depth):
-                r, p = f"{pre_ref}blocks.{i}.", f"{pre}blocks.{i}."
-                put(p + "n1_w", sd[r + "norm1.weight"]); put(p + "n2_w", sd[r + "norm2.weight"])
-                if ln:
-                    put(p + "n1_b", sd[r + "norm1.bias"]); put(p + "n2_b", sd[r + "norm2.bias"])
-                put(p + "qkv.w", sd[r + "attn.qkv.weight"]); put(p + "qkv.b", sd[r + "attn.qkv.bias"])
-                put(p + "proj.w", sd[r + "attn.proj.weight"]); put(p + "proj.b", sd[r + "attn.proj.bias"])
-                put(p + "fc1.w", E.interleave8(sd[r + "mlp.w1.weight"], sd[r + "mlp.w2.weight"]))
-                put(p + "fc1.b", E.interleave8(sd[r + "mlp.w1.bias"], sd[r + "mlp.w2.bias"]))
-                put(p + "fc2.w", sd[r + "mlp.w3.weight"]); put(p + "fc2.b", sd[r + "mlp.w3.bias"])
-            put(pre + "norm_w", sd[pre_ref + "norm.weight"])
-            if ln: put(pre + "norm_b", sd[pre_ref + "norm.bias"])
-
-        c = self.cfg
-        put("trunk.patch.w", sd["trunk.patch_embed.proj.weight"].flatten(1)); put("trunk.patch.b", sd["trunk.patch_embed.proj.bias"])
-        put("trunk.cls", sd["trunk.cls_token"]); put("trunk.mask_token", sd["trunk.mask_token"])
-        vit("trunk.", "trunk.", c.vision_depth, False)
-        put("trunk.bneck.w", sd["trunk.feature_bottleneck.weight"])
-        put("visual_proj.w", sd["visual_proj.weight"])
-        put("decoder.proj_in.w", sd["pixel_decoder.proj_in.weight"].flatten(1)); put("decoder.proj_in.b", sd["pixel_decoder.proj_in.bias"])
-        vit("pixel_decoder.", "decoder.", c.decoder_depth, True)
-        put("decoder.proj_out.w", sd["pixel_decoder.proj_out.weight"].flatten(1)); put("decoder.proj_out.b", sd["pixel_decoder.proj_out.bias"])
-        put("text.tok_emb", sd["token_embedding.weight"]); put("text.pos", sd["positional_embedding"])
-        for i in range(c.text_depth):
-            r, p = f"text_transformer.resblocks.{i}.", f"text.blocks.{i}."
-            put(p + "n1_w", sd[r + "ln_1.weight"]); put(p + "n1_b", sd[r + "ln_1.bias"])
-            put(p + "n2_w", sd[r + "ln_2.weight"]); put(p + "n2_b", sd[r + "ln_2.bias"])
-            put(p + "qkv.w", sd[r + "attn.in_proj_weight"]); put(p + "qkv.b", sd[r + "attn.in_proj_bias"])
-            put(p + "proj.w", sd[r + "attn.out_proj.weight"]); put(p + "proj.b", sd[r + "attn.out_proj.bias"])
-            put(p + "fc1.w", sd[r + "mlp.c_fc.weight"]); put(p + "fc1.b", sd[r + "mlp.c_fc.bias"])
-            put(p + "fc2.w", sd[r + "mlp.c_proj.weight"]); put(p + "fc2.b", sd[r + "mlp.c_proj.bias"])
-        put("text.norm_w", sd["ln_final.weight"]); put("text.norm_b", sd["ln_final.bias"])
-        put("text.proj.w", sd["text_projection"].t())
-        put("logit_scale", sd["logit_scale"].reshape(1))
-        if head_sd is not None:
-            for j in (0, 2, 4):
-                put(f"head.mlp{j}.w", head_sd[f"mlp.{j}.weight"]); put(f"head.mlp{j}.b", head_sd[f"mlp.{j}.bias"])
-            gk = "last_layer.weight_g" if "last_layer.weight_g" in head_sd else "last_layer.parametrizations.weight.original0"
-            vk = "last_layer.weight_v" if "last_layer.weight_v" in head_sd else "last_layer.parametrizations.weight.original1"
-            put("head.last_g", head_sd[gk].reshape(-1)); put("head.last_v", head_sd[vk])
-        st.sync_compute_copies(init_teacher=True)
+        P.import_reference(self.table, self.store.f32, sd, head_sd)
+        self.store.sync_compute_copies(init_teacher=True)
 
     @torch.no_grad()
     def export_state_dict(self) -> Dict[str, torch.Tensor]:
         """Student weights in the reference's VTPModel state-dict format."""
-        st, c = self.store, self.cfg
-        out = {}
-
-        def de8(t):
-            n = t.shape[0] // 2
-            v = t.reshape(n // 8, 2, 8, *t.shape[1:])
-            return v[:, 0].reshape(n, *t.shape[1:]).clone(), v[:, 1].reshape(n, *t.shape[1:]).clone()
-
-        def vit(pre_ref, pre, depth, ln):
-            for i in range(depth):
-                r, p = f"{pre_ref}blocks.{i}.", f"{pre}blocks.{i}."
-                out[r + "norm1.weight"] = st.f32(p + "n1_w").clone(); out[r + "norm2.weight"] = st.f32(p + "n2_w").clone()
-                if ln:
-                    out[r + "norm1.bias"] = st.f32(p + "n1_b").clone(); out[r + "norm2.bias"] = st.f32(p + "n2_b").clone()
-                out[r + "attn.qkv.weight"] = st.f32(p + "qkv.w").clone(); out[r + "attn.qkv.bias"] = st.f32(p + "qkv.b").clone()
-                out[r + "attn.proj.weight"] = st.f32(p + "proj.w").clone(); out[r + "attn.proj.bias"] = st.f32(p + "proj.b").clone()
-                out[r + "mlp.w1.weight"], out[r + "mlp.w2.weight"] = de8(st.f32(p + "fc1.w"))
-                out[r + "mlp.w1.bias"], out[r + "mlp.w2.bias"] = de8(st.f32(p + "fc1.b"))
-                out[r + "mlp.w3.weight"] = st.f32(p + "fc2.w").clone(); out[r + "mlp.w3.bias"] = st.f32(p + "fc2.b").clone()
-            out[pre_ref + "norm.weight"] = st.f32(pre + "norm_w").clone()
-            if ln: out[pre_ref + "norm.bias"] = st.f32(pre + "norm_b").clone()
-
-        ps = c.vision_patch_size
-        out["trunk.patch_embed.proj.weight"] = st.f32("trunk.patch.w").reshape(self.D, 3, ps, ps).clone()
-        out["trunk.patch_embed.proj.bias"] = st.f32("trunk.patch.b").clone()
-        out["trunk.cls_token"] = st.f32("trunk.cls").reshape(1, 1, -1).clone()
-        out["trunk.mask_token"] = st.f32("trunk.mask_token").reshape(1, -1).clone()
-        vit("trunk.", "trunk.", c.vision_depth, False)
-        out["trunk.feature_bottleneck.weight"] = st.f32("trunk.bneck.w").clone()
-        out["visual_proj.weight"] = st.f32("visual_proj.w").clone()
-        out["pixel_decoder.proj_in.weight"] = st.f32("decoder.proj_in.w").reshape(self.Dd, self.bn, 1, 1).clone()
-        out["pixel_decoder.proj_in.bias"] = st.f32("decoder.proj_in.b").clone()
-        vit("pixel_decoder.", "decoder.", c.decoder_depth, True)
-        out["pixel_decoder.proj_out.weight"] = st.f32("decoder.proj_out.w").reshape(768, self.Dd, 1, 1).clone()
-        out["pixel_decoder.proj_out.bias"] = st.f32("decoder.proj_out.b").clone()
-        out["token_embedding.weight"] = st.f32("text.tok_emb").clone(); out["positional_embedding"] = st.f32("text.pos").clone()
-        for i in range(c.text_depth):
-            r, p = f"text_transformer.resblocks.{i}.", f"text.blocks.{i}."
-            for a, b_ in (("ln_1.weight", "n1_w"), ("ln_1.bias", "n1_b"), ("ln_2.weight", "n2_w"), ("ln_2.bias", "n2_b"),
-                          ("attn.in_proj_weight", "qkv.w"), ("attn.in_proj_bias", "qkv.b"), ("attn.out_proj.weight", "proj.w"),
-                          ("attn.out_proj.bias", "proj.b"), ("mlp.c_fc.weight", "fc1.w"), ("mlp.c_fc.bias", "fc1.b"),
-                          ("mlp.c_proj.weight", "fc2.w"), ("mlp.c_proj.bias", "fc2.b")):
-                out[r + a] = st.f32(p + b_).clone()
-        out["ln_final.weight"] = st.f32("text.norm_w").clone(); out["ln_final.bias"] = st.f32("text.norm_b").clone()
-        out["text_projection"] = st.f32("text.proj.w").t().contiguous()
-        out["logit_scale"] = st.f32("logit_scale").reshape(()).clone()
-        from .rope import rope_periods
+        out = P.export_reference([e for e in self.table if not e.name.startswith("head.")], self.store.f32)
         out["trunk.rope_embed.periods"] = rope_periods(64).to(self.device)
         out["pixel_decoder.rope_embed.periods"] = rope_periods(64).to(self.device)
         return out
