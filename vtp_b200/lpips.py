@@ -26,6 +26,13 @@ VGG_CFG = [64, 64, "M", 128, 128, "M", 256, 256, 256, "M", 512, 512, 512, "M", 5
 TAPS = (1, 3, 6, 9, 12)  # conv indices whose ReLU output is a tap (relu1_2, 2_2, 3_3, 4_3, 5_3)
 
 
+def check_shape(H: int, W: int) -> None:
+    """Raise ValueError unless the VGG stack can run on H x W images: four 2x2 pools need H % 16 == 0, and the conv
+    GEMM needs every feature map's width to be a multiple of 4, so W % 64 == 0."""
+    if H % 16 or W % 64:
+        raise ValueError(f"LPIPS: {H}x{W} images are not supported (needs H % 16 == 0 and W % 64 == 0)")
+
+
 def _e(shape, dtype, dev):
     return torch.empty(shape, dtype=dtype, device=dev)
 
@@ -98,6 +105,7 @@ class LPIPSLoss:
         (coef = weight / batch gives the batch-mean LPIPS term of the reconstruction loss.)"""
         dev = self.device
         B, _, H, W = rec.shape
+        check_shape(H, W)
         dimg = _e((B, 3, H, W), F32, dev)
         for s in range(0, B, self.chunk):
             e = min(B, s + self.chunk)
@@ -162,9 +170,7 @@ class LPIPSMetric:
     forward only, fp32-accurate.  The reference runs the VGG in fp32 (TF32 convolutions under cuDNN's default); here
     every conv is the implicit-conv wgmma GEMM on bf16x3 operands (activations [hi|hi|lo] over 3C channels, weights
     [hi|lo|hi] per tap, fp32 accumulation and output with bias + ReLU), max-pool runs in fp32, and only the five taps
-    are kept.  Images are processed in chunks of `chunk` pairs to bound activation memory.
-
-    Shapes: the conv GEMM needs every feature map's width to be a multiple of 4, so H % 16 == 0 and W % 64 == 0."""
+    are kept.  Images are processed in chunks of `chunk` pairs to bound activation memory.  Shapes: see `check_shape`."""
 
     def __init__(self, vgg_w: Sequence[torch.Tensor], vgg_b: Sequence[torch.Tensor], lin_w: Sequence[torch.Tensor],
                  device="cuda", chunk: int = 8):
@@ -204,10 +210,7 @@ class LPIPSMetric:
         LPIPS lin file (keys lin{0..4}.model.1.weight; other keys are ignored, as the reference's strict=False load)."""
         return cls(*load_weight_files(vgg16_path, lin_path), device=device, chunk=chunk)
 
-    @staticmethod
-    def check_shape(H: int, W: int) -> None:
-        if H % 16 or W % 64:
-            raise ValueError(f"LPIPSMetric: {H}x{W} images are not supported (needs H % 16 == 0 and W % 64 == 0)")
+    check_shape = staticmethod(check_shape)
 
     def parts(self, lp: torch.Tensor) -> torch.Tensor:
         """lp fp32 [B, 2, 3, H, W] (the ScalingLayer outputs of each (reference, reconstruction) pair, as
