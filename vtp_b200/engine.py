@@ -321,16 +321,15 @@ def trunk_tokens(W: TowerW, img: torch.Tensor, mode: str, mask_idx: Optional[tor
 
 def trunk_forward(W: TowerW, img: torch.Tensor, mode: str, *, mask_idx=None, tape: Optional[dict] = None,
                   taps=None, drop: Optional[DropPlan] = None, hook=None):
-    """encoders/vision_transformer.py:221-258 for one resolution group.  Returns (x_prenorm [B*T,D] fp32, meta)."""
+    """encoders/vision_transformer.py:221-258 for one resolution group.  Returns (x_prenorm [B*T,D] fp32, meta).
+    A tape dict is filled with what train.trunk_backward reads: patch_a, mask_idx, the block tape, x (the stream the
+    final norm reads: pass the same tape to that norm for its statistics) and meta."""
     x, (B, T, gh, gw), a = trunk_tokens(W, img, mode, mask_idx)
-    if tape is not None:
-        tape["patch_a"] = a
     rope = W.rope(gh, gw, img.device)
     blk_tape = [] if tape is not None else None
     x = tower_blocks(W, x, B, T, rope, mode, tape=blk_tape, taps=taps, drop=drop, hook=hook)
     if tape is not None:
-        tape["blocks"] = blk_tape
-        tape["meta"] = (B, T, gh, gw)
+        tape.update(patch_a=a, mask_idx=mask_idx, blocks=blk_tape, x=x, meta=(B, T, gh, gw))
     return x, (B, T, gh, gw)
 
 
@@ -361,38 +360,44 @@ def latents_nchw(patch_tokens: torch.Tensor, gh: int, gw: int) -> torch.Tensor:
 
 
 # ------------------------------------------------------------------------------------------------------ pixel decoder
-def decoder_forward(W: TowerW, lat: torch.Tensor, mode: str, *, tape: Optional[dict] = None) -> torch.Tensor:
+def decoder_forward(W: TowerW, lat: torch.Tensor, mode: str) -> torch.Tensor:
     """decoders/pixel_decoder.py:134-162: latents [B, C, h, w] -> image [B, 3, 16h, 16w]."""
-    dev = lat.device
     B, C, gh, gw = lat.shape
-    HW, D = gh * gw, W.D
-    M = B * HW
-    act = BF if mode == "bf16" else F32
     lat = lat.contiguous()
     if lat.dtype not in (BF, F32):
         lat = lat.to(F32)
-    tok = _e((M, C), act, dev)  # (B,C,HW) -> (B,HW,C): flatten(2).transpose(1,2)
-    lib.transpose_batched(lat, tok, B, C, HW)
+    tok = _e((B * gh * gw, C), BF if mode == "bf16" else F32, lat.device)  # flatten(2).transpose(1,2)
+    lib.transpose_batched(lat, tok, B, C, gh * gw)
+    return decoder_tokens(W, tok, (B, gh, gw), mode)
+
+
+def decoder_tokens(W: TowerW, tok: torch.Tensor, grid: Tuple[int, int, int], mode: str, *,
+                   tape: Optional[dict] = None) -> torch.Tensor:
+    """The decoder on token-major latents tok [B*h*w, C] of grid (B, h, w): proj_in, blocks, norm, proj_out with the
+    PixelShuffle store -> image [B, 3, r h, r w].  A tape dict is filled with what train.decoder_backward reads: tok,
+    the block tape, x (the stream before the norm), rstd / mean, xn (the norm output) and meta."""
+    B, gh, gw = grid
+    M, D, dev = B * gh * gw, W.D, tok.device
     pin: Lin = W.extra["proj_in"]
     x = _e((M, D), BF if W.stream_bf16 else F32, dev)
-    linear(operand(tok, M, C, mode), pin, x, M, mode)
-    rope = W.rope(gh, gw, dev)
+    linear(operand(tok, M, tok.shape[1], mode), pin, x, M, mode)
     blk_tape = [] if tape is not None else None
-    x = tower_blocks(W, x, B, HW, rope, mode, tape=blk_tape)
-    nt = {} if tape is not None else None
-    xn = norm(x, M, D, W.norm_w, W.norm_b, W.eps, mode, want="op", tape=nt)
+    x = tower_blocks(W, x, B, gh * gw, W.rope(gh, gw, dev), mode, tape=blk_tape)
+    xn = norm(x, M, D, W.norm_w, W.norm_b, W.eps, mode, want="op", tape=tape)
     pout: Lin = W.extra["proj_out"]
     r = int(round((pout.N // 3) ** 0.5))
-    img = _e((B, 3, gh * r, gw * r), act, dev)
+    img = _e((B, 3, gh * r, gw * r), BF if mode == "bf16" else F32, dev)
     linear(xn, pout, img, M, mode, pixel_shuffle=(r, gh, gw, 3), ldo=gw * r)
     if tape is not None:
-        tape.update(blocks=blk_tape, meta=(B, HW, gh, gw), tok=tok, x_final=x, xn=xn, nf=nt)
+        tape.update(tok=tok, blocks=blk_tape, x=x, xn=xn, meta=(B, gh * gw, gh, gw))
     return img
 
 
 # ------------------------------------------------------------------------------------------------------ text tower
 def text_forward(W: TowerW, ids: torch.Tensor, mode: str, *, tape: Optional[dict] = None) -> torch.Tensor:
-    """vtp_hf/modeling_vtp.py:278-310 up to (not including) the final normalize: ids int64 [B, L] -> [B, E]."""
+    """vtp_hf/modeling_vtp.py:278-310 up to (not including) the final normalize: ids int64 [B, L] -> [B, E].  A tape
+    dict is filled with what train.text_backward reads: ids, the block tape, x (the stream before the final norm),
+    rstd / mean, eot, pooled and meta."""
     dev = ids.device
     B, L = ids.shape
     D = W.D
@@ -402,8 +407,7 @@ def text_forward(W: TowerW, ids: torch.Tensor, mode: str, *, tape: Optional[dict
     lib.embed_tokens(ids, W.extra["tok_emb"], W.extra["pos"], x)
     blk_tape = [] if tape is not None else None
     x = tower_blocks(W, x, B, L, None, mode, causal=True, tape=blk_tape)
-    nt = {} if tape is not None else None
-    xn = norm(x, M, D, W.norm_w, W.norm_b, W.eps, mode, want="f32", tape=nt)
+    xn = norm(x, M, D, W.norm_w, W.norm_b, W.eps, mode, want="f32", tape=tape)
     # text_global_pool 'argmax' (encoders/text_transformer.py:222-224): integer index glue, bit-exact
     eot = ids.argmax(dim=-1) + torch.arange(B, device=dev) * L
     act = BF if mode == "bf16" else F32
@@ -413,7 +417,7 @@ def text_forward(W: TowerW, ids: torch.Tensor, mode: str, *, tape: Optional[dict
     f = _e((B, proj.N), act, dev)
     linear(operand(pooled, B, D, mode), proj, f, B, mode)
     if tape is not None:
-        tape.update(blocks=blk_tape, meta=(B, L), x_final=x, nf=nt, eot=eot, pooled=pooled)
+        tape.update(ids=ids, blocks=blk_tape, x=x, eot=eot, pooled=pooled, meta=(B, L))
     return f
 
 

@@ -201,6 +201,68 @@ def tower_blocks_backward(W: TowerW, G: TowerW, tape: list, g: torch.Tensor, B: 
     return g
 
 
+def trunk_backward(W: TowerW, G: TowerW, tape: dict, dxn: torch.Tensor, g: Optional[torch.Tensor] = None):
+    """Reverse of engine.trunk_forward and the final norm from their tape: dxn (bf16 dL/d(final-norm output) [B*T, D])
+    -> accumulates every trunk parameter gradient.  g: zeroed fp32 [B*T, D] to differentiate the stream into (a fresh
+    one if None)."""
+    B, T, gh, gw = tape["meta"]
+    D, HW, M, dev = W.D, gh * gw, B * T, dxn.device
+    if g is None:
+        g = torch.zeros((M, D), dtype=F32, device=dev)
+    lib.norm_bwd(tape["x"], tape["rstd"], tape["mean"], W.norm_w, dxn, g, G.norm_w, G.norm_b, M, D)
+    tower_blocks_backward(W, G, tape["blocks"], g, B, T, W.rope(gh, gw, dev))
+    gp = _e((B * HW, D), BF, dev)
+    lib.strip_prefix(g, gp, G.extra["cls"], B, T, 1, D)
+    mask_idx = tape["mask_idx"]
+    if mask_idx is not None and mask_idx.numel() > 0:
+        rows = (mask_idx // HW) * T + 1 + mask_idx % HW
+        tmp = _e((mask_idx.numel(), D), F32, dev)
+        lib.gather_rows(g, tmp, rows, D)
+        lib.cast_colsum(tmp, None, G.extra["mask_token"], mask_idx.numel(), D)
+        zeros = torch.zeros(D, dtype=F32, device=dev)
+        lib.apply_mask_tokens(gp, zeros, mask_idx, HW, HW, 0, D)
+    wgrad(gp, tape["patch_a"], G.extra["patch"].w, B * HW)
+    lib.cast_colsum(gp, None, G.extra["patch"].b, B * HW, D)
+
+
+def decoder_backward(W: TowerW, G: TowerW, tape: dict, dY: torch.Tensor, dtok: torch.Tensor, **row_map):
+    """Reverse of engine.decoder_tokens from its tape: dY (bf16 dL/d(proj_out output) [B*h*w, 3r²]) -> dtok
+    (dL/d(tok), written through the caller's `row_map` GEMM epilogue arguments); accumulates every decoder gradient."""
+    B, HW, gh, gw = tape["meta"]
+    D, M, dev = W.D, B * HW, dY.device
+    pout, pin = W.extra["proj_out"], W.extra["proj_in"]
+    dxn = _e((M, D), BF, dev)
+    dgrad(dY, pout.w, dxn, M)
+    wgrad(dY, tape["xn"], G.extra["proj_out"].w, M)
+    lib.cast_colsum(dY, None, G.extra["proj_out"].b, M, pout.N)
+    g = torch.zeros((M, D), dtype=F32, device=dev)
+    lib.norm_bwd(tape["x"], tape["rstd"], tape["mean"], W.norm_w, dxn, g, G.norm_w, G.norm_b, M, D)
+    tower_blocks_backward(W, G, tape["blocks"], g, B, HW, W.rope(gh, gw, dev))
+    gb = _e((M, D), BF, dev)
+    lib.cast_colsum(g, gb, G.extra["proj_in"].b, M, D)
+    dgrad(gb, pin.w, dtok, M, **row_map)
+    wgrad(gb, tape["tok"], G.extra["proj_in"].w, M)
+
+
+def text_backward(W: TowerW, G: TowerW, tape: dict, dft_raw: torch.Tensor):
+    """Reverse of engine.text_forward from its tape: dft_raw (bf16 dL/d(projected feature) [B, E]) -> accumulates
+    every text-tower parameter gradient."""
+    B, L = tape["meta"]
+    D, M, dev = W.D, B * L, dft_raw.device
+    dpool = _e((B, D), F32, dev)
+    dgrad(dft_raw, W.extra["proj"].w, dpool, B)
+    wgrad(dft_raw, tape["pooled"], G.extra["proj"].w, B)
+    dxn32 = torch.zeros((M, D), dtype=F32, device=dev)
+    lib.scatter_add_rows(dpool, dxn32, tape["eot"], D)
+    dxn = _e((M, D), BF, dev)
+    lib.cast_colsum(dxn32, dxn, None, M, D)
+    g = torch.zeros((M, D), dtype=F32, device=dev)
+    lib.norm_bwd(tape["x"], tape["rstd"], tape["mean"], W.norm_w, dxn, g, G.norm_w, G.norm_b, M, D)
+    tower_blocks_backward(W, G, tape["blocks"], g, B, L, None, causal=True)
+    lib.scatter_add_rows(g, G.extra["tok_emb"], tape["ids"].reshape(-1), D)
+    lib.cast_colsum(g, None, G.extra["pos"].view(-1), B, L * D, ldx=L * D)
+
+
 def grad_buckets(offset: Dict[str, int], n: int) -> Dict[str, List[Tuple[int, int]]]:
     """Contiguous ranges of the flat gradient buffer per tower.  A tower's gradient is FINAL as soon as its last
     backward of the step has run: text tower + clip projection + logit scale after the contrastive objective, DINO head
@@ -287,7 +349,7 @@ class VTPTrainer:
             raise NotImplementedError("the trainer projects the trunk's cls token, not its bottleneck features, for the "
                                       "contrastive objective (vision_bottleneck_ae_only=True)")
         check_head_dims(c)
-        self.D, self.Dd, self.Dt = c.vision_embed_dim, c.decoder_embed_dim, c.text_embed_dim
+        self.D, self.Dt = c.vision_embed_dim, c.text_embed_dim
         self.hs = P.geometry(c, "trunk").hidden
         self.bn = c.vision_feature_bottleneck
         K, hb = self.tc.head_out_dim, self.tc.head_bottleneck
@@ -398,29 +460,6 @@ class VTPTrainer:
         preset = self.drop_presets.pop(0) if getattr(self, "drop_presets", None) else None
         return E.DropPlan(ratio, self.world, self.rank, preset=preset)
 
-    def _trunk_fwd(self, W: TowerW, img, tape: Optional[dict], mask_idx=None, drop=None):
-        x, meta = E.trunk_forward(W, img, "bf16", mask_idx=mask_idx, tape=tape, drop=drop)
-        return x, meta
-
-    def _trunk_bwd(self, tape: dict, g: torch.Tensor, mask_idx=None):
-        """g fp32 [B*T, D] = dL/d(x_prenorm) -> accumulates all trunk parameter gradients."""
-        W, G = self.towers[("trunk", "param")], self.towers[("trunk", "grad")]
-        B, T, gh, gw = tape["meta"]
-        D, HW = W.D, gh * gw
-        rope = W.rope(gh, gw, g.device)
-        tower_blocks_backward(W, G, tape["blocks"], g, B, T, rope)
-        gp = _e((B * HW, D), BF, g.device)
-        lib.strip_prefix(g, gp, G.extra["cls"], B, T, 1, D)
-        if mask_idx is not None and mask_idx.numel() > 0:
-            rows = (mask_idx // HW) * T + 1 + mask_idx % HW
-            tmp = _e((mask_idx.numel(), D), F32, g.device)
-            lib.gather_rows(g, tmp, rows, D)
-            lib.cast_colsum(tmp, None, G.extra["mask_token"], mask_idx.numel(), D)
-            zeros = torch.zeros(D, dtype=F32, device=g.device)
-            lib.apply_mask_tokens(gp, zeros, mask_idx, HW, HW, 0, D)
-        wgrad(gp, tape["patch_a"], G.extra["patch"].w, B * HW)
-        lib.cast_colsum(gp, None, G.extra["patch"].b, B * HW, D)
-
     # -------------------------------------------------------------- objective 1: CLIP (vtp.py:340-363 + ClipLoss)
     def clip_fwd_bwd(self, image: torch.Tensor, text: torch.Tensor, weight: float = 1.0):
         import torch.distributed as dist
@@ -430,10 +469,8 @@ class VTPTrainer:
         D, Dt = self.D, self.Dt
         # ---- image tower -> cls -> visual_proj -> normalise
         tp_i = {}
-        x, (B, T, gh, gw) = self._trunk_fwd(W, image, tp_i, drop=self._drop(self.tc.clip_drop_rate))
-        M = B * T
-        nt = {}
-        xn = E.norm(x, M, D, W.norm_w, None, W.eps, "bf16", want="f32", tape=nt)
+        x, (B, T, gh, gw) = E.trunk_forward(W, image, "bf16", tape=tp_i, drop=self._drop(self.tc.clip_drop_rate))
+        xn = E.norm(x, B * T, D, W.norm_w, None, W.eps, "bf16", want="f32", tape=tp_i)
         cls_rows = torch.arange(B, device=dev, dtype=torch.long) * T
         cls = _e((B, D), BF, dev)
         lib.gather_rows(xn, cls, cls_rows, D)
@@ -447,7 +484,7 @@ class VTPTrainer:
         nrm_t = _e((B,), F32, dev)
         if self._clip_exchange() == "p2p":
             dfi, dft = self._clip_loss_p2p(fi_raw, ft_raw, nrm_i, nrm_t, B, weight)
-            self._clip_backward(tp_i, tp_t, x, nt, cls, self.peer.img, self.peer.txt, nrm_i, nrm_t, dfi, dft, text, B, T)
+            self._clip_backward(tp_i, tp_t, cls, self.peer.img, self.peer.txt, nrm_i, nrm_t, dfi, dft)
             return
         fi = torch.empty_like(fi_raw)
         lib.l2norm_fwd(fi_raw, fi, B, Dt, 1e-12, norm_out=nrm_i)
@@ -493,7 +530,7 @@ class VTPTrainer:
         else:
             lib.gemm(Gt_, ft, dfi, M=B, N=Dt, K=B, a_mn=True, b_mn=True, lda=Bgp, ldb=Dt, accumulate=True, round_bf16=False)
             lib.gemm(Gi, fi, dft, M=B, N=Dt, K=B, a_mn=True, b_mn=True, lda=Bgp, ldb=Dt, accumulate=True, round_bf16=False)
-        self._clip_backward(tp_i, tp_t, x, nt, cls, fi, ft, nrm_i, nrm_t, dfi, dft, text, B, T)
+        self._clip_backward(tp_i, tp_t, cls, fi, ft, nrm_i, nrm_t, dfi, dft)
 
     def _clip_exchange(self) -> str:
         import os
@@ -539,45 +576,21 @@ class VTPTrainer:
         lib.gemm(dMt, fi_all, dft, M=B, N=Dt, K=Bgp, b_mn=True, ldb=Dt, round_bf16=False)
         return dfi, dft
 
-    def _clip_backward(self, tp_i, tp_t, x, nt, cls, fi, ft, nrm_i, nrm_t, dfi, dft, text, B: int, T: int):
+    def _clip_backward(self, tp_i, tp_t, cls, fi, ft, nrm_i, nrm_t, dfi, dft):
+        """dfi / dft (fp32 dL/d(normalised feature)) back through the L2 norms, the image head and both towers."""
         dev = self.device
         W, G = self.towers[("trunk", "param")], self.towers[("trunk", "grad")]
+        B, T = tp_i["meta"][:2]
         D, Dt = self.D, self.Dt
-        M = B * T
-        vp: Lin = W.extra["visual_proj"]
-        # ---- image side backward
         dfi_raw = _e((B, Dt), BF, dev)
         lib.l2norm_bwd(fi, nrm_i, dfi, dfi_raw, B, Dt)
-        dxn = torch.zeros((M, D), dtype=BF, device=dev)
-        dgrad(dfi_raw, vp.w, dxn, B, ldo=T * D)          # row b of d(cls) lands on token row b*T
+        dxn = torch.zeros((B * T, D), dtype=BF, device=dev)
+        dgrad(dfi_raw, W.extra["visual_proj"].w, dxn, B, ldo=T * D)   # row b of d(cls) lands on token row b*T
         wgrad(dfi_raw, cls, G.extra["visual_proj"].w, B)
-        g = torch.zeros((M, D), dtype=F32, device=dev)
-        lib.norm_bwd(x, nt["rstd"], None, W.norm_w, dxn, g, G.norm_w, None, M, D)
-        self._trunk_bwd(tp_i, g)
-        # ---- text side backward
-        self._text_bwd(tp_t, ft, nrm_t, dft, text)
-
-    def _text_bwd(self, tape, ft, nrm_t, dft, ids):
-        dev = self.device
-        Wt, Gt = self.towers[("text", "param")], self.towers[("text", "grad")]
-        B, L = tape["meta"]
-        Dt, M = self.Dt, B * L
+        trunk_backward(W, G, tp_i, dxn)
         dft_raw = _e((B, Dt), BF, dev)
         lib.l2norm_bwd(ft, nrm_t, dft, dft_raw, B, Dt)
-        proj: Lin = Wt.extra["proj"]
-        dpool = _e((B, Dt), F32, dev)
-        dgrad(dft_raw, proj.w, dpool, B)
-        wgrad(dft_raw, tape["pooled"], Gt.extra["proj"].w, B)
-        dxn32 = torch.zeros((M, Dt), dtype=F32, device=dev)
-        lib.scatter_add_rows(dpool, dxn32, tape["eot"], Dt)
-        dxn = _e((M, Dt), BF, dev)
-        lib.cast_colsum(dxn32, dxn, None, M, Dt)
-        g = torch.zeros((M, Dt), dtype=F32, device=dev)
-        nf = tape["nf"]
-        lib.norm_bwd(tape["x_final"], nf["rstd"], nf["mean"], Wt.norm_w, dxn, g, Gt.norm_w, Gt.norm_b, M, Dt)
-        tower_blocks_backward(Wt, Gt, tape["blocks"], g, B, L, None, causal=True)
-        lib.scatter_add_rows(g, Gt.extra["tok_emb"], ids.reshape(-1), Dt)
-        lib.cast_colsum(g, None, Gt.extra["pos"].view(-1), B, L * Dt, ldx=L * Dt)
+        text_backward(self.towers[("text", "param")], self.towers[("text", "grad")], tp_t, dft_raw)
 
     # -------------------------------------------------------------- objective 3: reconstruction (vtp.py:487-512)
     def rec_fwd_bwd(self, image: torch.Tensor, weight: float = 1.0, return_image: bool = False,
@@ -586,59 +599,33 @@ class VTPTrainer:
         dev = self.device
         W, G = self.towers[("trunk", "param")], self.towers[("trunk", "grad")]
         Wd, Gd = self.towers[("decoder", "param")], self.towers[("decoder", "grad")]
-        D, Dd, bn = self.D, self.Dd, self.bn
-        tp_e = {}
-        x, (B, T, gh, gw) = self._trunk_fwd(W, image, tp_e, drop=self._drop(self.tc.rec_drop_rate))
+        D, bn = self.D, self.bn
+        tp_e, tp_d = {}, {}
+        x, (B, T, gh, gw) = E.trunk_forward(W, image, "bf16", tape=tp_e, drop=self._drop(self.tc.rec_drop_rate))
         M, HW = B * T, gh * gw
-        Md = B * HW
         nB = norm_B if norm_B is not None else B
-        nt = {}
-        xn = E.norm(x, M, D, W.norm_w, None, W.eps, "bf16", want="op", tape=nt)
+        xn = E.norm(x, M, D, W.norm_w, None, W.eps, "bf16", want="op", tape=tp_e)
         bneck: Lin = W.extra["bneck"]
-        tok = _e((Md, bn), BF, dev)                      # latents as decoder tokens (cls rows dropped in the epilogue)
+        tok = _e((B * HW, bn), BF, dev)                  # latents as decoder tokens (cls rows dropped in the epilogue)
         lib.gemm(xn, bneck.w, tok, M=M, N=bn, K=D, rr_group=T, rr_skip=-1)
-        # ---- decoder (decoders/pixel_decoder.py:134-162) on token-major latents
-        pin: Lin = Wd.extra["proj_in"]
-        xd = _e((Md, Dd), BF, dev)
-        lib.gemm(tok, pin.w, xd, M=Md, N=Dd, K=bn, bias=pin.b)
-        rope = Wd.rope(gh, gw, dev)
-        dtape = []
-        xd = E.tower_blocks(Wd, xd, B, HW, rope, "bf16", tape=dtape)
-        ntd = {}
-        xdn = E.norm(xd, Md, Dd, Wd.norm_w, Wd.norm_b, Wd.eps, "bf16", want="op", tape=ntd)
-        pout: Lin = Wd.extra["proj_out"]
-        r = 16
-        rec = _e((B, 3, gh * r, gw * r), BF, dev)
-        lib.gemm(xdn, pout.w, rec, M=Md, N=pout.N, K=Dd, bias=pout.b, pixel_shuffle=(r, gh, gw, 3), ldo=gw * r)
+        rec = E.decoder_tokens(Wd, tok, (B, gh, gw), "bf16", tape=tp_d)
+        r = rec.shape[-1] // gw
         # ---- loss: L1 (+ LPIPS gradient if a perceptual module is attached)
         dlp = None
         if getattr(self, "lpips", None) is not None and self.tc.lpips_weight > 0:
             dlp = self.lpips.loss_and_grad(rec, image, weight * self.tc.lpips_weight / nB, self.loss_acc[5:6])
-        dY = _e((Md, pout.N), BF, dev)
+        dY = _e((B * HW, 3 * r * r), BF, dev)
         lib.recon_l1_grad(rec, image.contiguous(), dlp, dY, self.loss_acc[4:5], B, 3, gh, gw, r,
                           weight / (rec.numel() // B * nB))
-        # ---- decoder backward
-        dxdn = _e((Md, Dd), BF, dev)
-        dgrad(dY, pout.w, dxdn, Md)
-        wgrad(dY, xdn, Gd.extra["proj_out"].w, Md)
-        lib.cast_colsum(dY, None, Gd.extra["proj_out"].b, Md, pout.N)
-        g = torch.zeros((Md, Dd), dtype=F32, device=dev)
-        lib.norm_bwd(xd, ntd["rstd"], ntd["mean"], Wd.norm_w, dxdn, g, Gd.norm_w, Gd.norm_b, Md, Dd)
-        tower_blocks_backward(Wd, Gd, dtape, g, B, HW, rope)
-        gb = _e((Md, Dd), BF, dev)
-        lib.cast_colsum(g, gb, Gd.extra["proj_in"].b, Md, Dd)
         dz = torch.zeros((M, bn), dtype=BF, device=dev)  # d(latent tokens), re-expanded to [B*T] rows (cls rows = 0)
-        dgrad(gb, pin.w, dz, Md, rr_group=HW, rr_skip=1)
-        wgrad(gb, tok, Gd.extra["proj_in"].w, Md)
+        decoder_backward(Wd, Gd, tp_d, dY, dz, rr_group=HW, rr_skip=1)
         if final_group:
             self._reduce_bucket("decoder")   # pixel-decoder gradient is final: all-reduce under the encoder backward
         # ---- encoder side
         dxn = _e((M, D), BF, dev)
         dgrad(dz, bneck.w, dxn, M)
         wgrad(dz, xn, G.extra["bneck"].w, M)
-        ge = torch.zeros((M, D), dtype=F32, device=dev)
-        lib.norm_bwd(x, nt["rstd"], None, W.norm_w, dxn, ge, G.norm_w, None, M, D)
-        self._trunk_bwd(tp_e, ge)
+        trunk_backward(W, G, tp_e, dxn)
         return rec if return_image else None
 
     # -------------------------------------------------------------- DINO head (heads/dino_head.py:65-126)
@@ -773,7 +760,7 @@ class VTPTrainer:
         B = B2 // 2
         n_m = mask_indices.numel()
         # ---------------- teacher (no grad): get_teacher_forward_outputs vtp.py:410-450
-        xt, (_, T, gh, gw) = self._trunk_fwd(Wt, global_crops, None)
+        xt, (_, T, gh, gw) = E.trunk_forward(Wt, global_crops, "bf16")
         HW = gh * gw
         xnt = E.norm(xt, B2 * T, D, Wt.norm_w, None, Wt.eps, "bf16", want="f32")
         ar = torch.arange(B2, device=dev, dtype=torch.long)
@@ -794,11 +781,11 @@ class VTPTrainer:
         del xt, xnt
         # ---------------- student: get_student_ssl_outputs vtp.py:452-484
         tp_g, tp_l = {}, {}
-        xg, _ = self._trunk_fwd(W, global_crops, tp_g, mask_idx=mask_indices, drop=self._drop(tc.ssl_drop_rate))
-        xl, (Bl, Tl, ghl, gwl) = self._trunk_fwd(W, local_crops, tp_l, drop=self._drop(tc.ssl_drop_rate))
-        ntg, ntl = {}, {}
-        xng = E.norm(xg, B2 * T, D, W.norm_w, None, W.eps, "bf16", want="f32", tape=ntg)
-        xnl = E.norm(xl, Bl * Tl, D, W.norm_w, None, W.eps, "bf16", want="f32", tape=ntl)
+        xg, _ = E.trunk_forward(W, global_crops, "bf16", mask_idx=mask_indices, tape=tp_g,
+                                drop=self._drop(tc.ssl_drop_rate))
+        xl, (Bl, Tl, _, _) = E.trunk_forward(W, local_crops, "bf16", tape=tp_l, drop=self._drop(tc.ssl_drop_rate))
+        xng = E.norm(xg, B2 * T, D, W.norm_w, None, W.eps, "bf16", want="f32", tape=tp_g)
+        xnl = E.norm(xl, Bl * Tl, D, W.norm_w, None, W.eps, "bf16", want="f32", tape=tp_l)
         l_rows = torch.arange(Bl, device=dev, dtype=torch.long) * Tl
         Ts = Bl + B2 + n_m
         sin_ = _e((Ts, D), BF, dev)
@@ -831,17 +818,13 @@ class VTPTrainer:
         lib.scatter_add_rows(dsin[:Bl], dl32, l_rows, D)
         dxl = _e((Bl * Tl, D), BF, dev)
         lib.cast_colsum(dl32, dxl, None, Bl * Tl, D)
-        gl = dl32.zero_()
-        lib.norm_bwd(xl, ntl["rstd"], None, W.norm_w, dxl, gl, G.norm_w, None, Bl * Tl, D)
-        self._trunk_bwd(tp_l, gl)
-        del gl, dl32, dxl, xl, xnl, tp_l
+        trunk_backward(W, G, tp_l, dxl, dl32.zero_())
+        del dl32, dxl, xl, xnl, tp_l
         dg32 = torch.zeros((B2 * T, D), dtype=F32, device=dev)
         lib.scatter_add_rows(dsin[Bl:], dg32, torch.cat([cls_rows, m_rows]), D)
         dxg = _e((B2 * T, D), BF, dev)
         lib.cast_colsum(dg32, dxg, None, B2 * T, D)
-        gg = dg32.zero_()
-        lib.norm_bwd(xg, ntg["rstd"], None, W.norm_w, dxg, gg, G.norm_w, None, B2 * T, D)
-        self._trunk_bwd(tp_g, gg, mask_idx=mask_indices)
+        trunk_backward(W, G, tp_g, dxg, dg32.zero_())
 
     # -------------------------------------------------------------- optimiser (+ EMA teacher, vtp.py:388-401)
     def allreduce_grads(self):
