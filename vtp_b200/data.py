@@ -120,6 +120,10 @@ class TrainBatchPipeline:
         for ...:
             batch = pipe.get(); pipe.submit(next_images, next_captions)   # prepared under the step that follows
             trainer.train_step(batch)               # or replay_step(batch)
+
+    `state_dict()` / `load_state_dict()` carry the RNG streams over a restart (`VTPTrainer.save_checkpoint(path,
+    pipeline=pipe)` stores them): the resumed pipeline, given the images of the batches that were still queued, prepares
+    them bit for bit as this one did.
     """
 
     def __init__(self, device="cuda", *, image_size: int = 256, local_size: int = 96, n_local: int = 8, patch: int = 16,
@@ -143,7 +147,31 @@ class TrainBatchPipeline:
         self._mean_ws: Dict[int, torch.Tensor] = {}
         self.stream = torch.cuda.Stream(self.device)
         self.pool = ThreadPoolExecutor(max_workers=1)
-        self._queue: List[Tuple[Dict[str, torch.Tensor], torch.cuda.Event, Optional[Future]]] = []
+        # (batch, ready event, caption future, RNG state before the batch's draws)
+        self._queue: List[Tuple[Dict[str, torch.Tensor], torch.cuda.Event, Optional[Future], dict]] = []
+
+    def _rng_state(self) -> dict:
+        return {"rng": self.rng.bit_generator.state, "photo_rng": self.photo_rng.bit_generator.state,
+                "gen": bytes(self.gen.get_state().numpy())}
+
+    def state_dict(self) -> dict:
+        """The RNG streams (boxes and flips, photometric rows, iBOT masks) as they were before the oldest batch not yet
+        returned by get(), or as they are now when none is queued: a pipeline that loads this state and is given the
+        images of the batches still queued here, in order, prepares them bit for bit as this one does.  The NumPy states
+        are JSON-serialisable dicts, the CUDA generator's state is bytes."""
+        return self._queue[0][3] if self._queue else self._rng_state()
+
+    def check_loadable(self) -> None:
+        if self._queue:
+            raise ValueError(f"load_state_dict() with {len(self._queue)} batch(es) queued: they were drawn from the "
+                             f"current streams; get() them first")
+
+    def load_state_dict(self, state: dict) -> None:
+        """Restore state_dict()'s RNG streams; the next submit() draws what the saving pipeline drew for its batch."""
+        self.check_loadable()
+        self.rng.bit_generator.state = state["rng"]
+        self.photo_rng.bit_generator.state = state["photo_rng"]
+        self.gen.set_state(torch.frombuffer(bytearray(state["gen"]), dtype=torch.uint8))
 
     def _crops(self, src: torch.Tensor, n_per: int, size: int, scale, norm, flip: bool = True,
                photo: Optional[np.ndarray] = None) -> torch.Tensor:
@@ -171,6 +199,7 @@ class TrainBatchPipeline:
     def submit(self, images_u8: torch.Tensor, captions=None) -> None:
         """images_u8: uint8 [B, H, W, 3]; captions: list[str] (needs `tokenizer`) or int64 ids [B, L] or None."""
         assert images_u8.dtype == torch.uint8 and images_u8.dim() == 4 and images_u8.shape[-1] == 3
+        state = self._rng_state()
         fut = None
         ids = None
         if captions is not None and not torch.is_tensor(captions):
@@ -203,10 +232,10 @@ class TrainBatchPipeline:
             src.record_stream(self.stream)
             ev = torch.cuda.Event()
             ev.record(self.stream)
-        self._queue.append((batch, ev, fut))
+        self._queue.append((batch, ev, fut, state))
 
     def get(self) -> Dict[str, torch.Tensor]:
-        batch, ev, fut = self._queue.pop(0)
+        batch, ev, fut, _ = self._queue.pop(0)
         if fut is not None:
             batch["text"] = fut.result().to(self.device, non_blocking=True)
         torch.cuda.current_stream(self.device).wait_event(ev)

@@ -7,6 +7,8 @@ update_teacher) plus the loss / optimiser layer that the reference does not rele
     (`ParamStore`); GEMM weights are stored in kernel layout (w1|w2 8-interleaved for the SwiGLU-gate epilogue);
     `import_state_dict` / `export_state_dict` convert from/to the reference's state-dict keys;
   * one fused kernel per region does AdamW + bf16 refresh + EMA teacher (vtp.py:388-401) + gradient zeroing;
+  * `save_checkpoint` / `load_checkpoint` write and restore the whole training state (format: checkpoint.py) in place,
+    under a captured step graph too;
   * data parallel: gradients are all-reduced (NCCL) on the flat buffer, contrastive features are all-gathered and
     their gradients reduced back — the only two collectives on the path (SURVEY.md §8e).
 Precision is the reference-under-autocast ("bf16") mode throughout.
@@ -76,6 +78,8 @@ class ParamStore:
     def f32(self, name): return self._view(self.p, name)
     def bf16(self, name): return self._view(self.pb, name)
     def grad(self, name): return self._view(self.g, name)
+    def exp_avg(self, name): return self._view(self.m, name)
+    def exp_avg_sq(self, name): return self._view(self.v, name)
     def tf32(self, name): return self._view(self.tp, name)
     def tbf16(self, name): return self._view(self.tpb, name)
 
@@ -444,12 +448,74 @@ class VTPTrainer:
         self.store.sync_compute_copies(init_teacher=True)
 
     @torch.no_grad()
-    def export_state_dict(self) -> Dict[str, torch.Tensor]:
-        """Student weights in the reference's VTPModel state-dict format."""
-        out = P.export_reference([e for e in self.table if not e.name.startswith("head.")], self.store.f32)
+    def export_state_dict(self, teacher: bool = False) -> Dict[str, torch.Tensor]:
+        """Student weights in the reference's VTPModel state-dict format.  teacher=True takes the trunk and the clip
+        projection from the EMA teacher instead (what DINOv2-style evaluation scores); the pixel decoder and the text
+        tower, which the teacher does not have, still come from the student."""
+        st = self.store
+        ema = {e.name for e in self.table if e.teacher} if teacher else set()
+        out = P.export_reference([e for e in self.table if not e.name.startswith("head.")],
+                                 lambda name: st.tf32(name) if name in ema else st.f32(name))
         out["trunk.rope_embed.periods"] = rope_periods(64).to(self.device)
         out["pixel_decoder.rope_embed.periods"] = rope_periods(64).to(self.device)
         return out
+
+    # -------------------------------------------------------------- checkpoints (format: checkpoint.py)
+    def _checkpoint_tensors(self) -> Dict[str, torch.Tensor]:
+        """Views of every buffer a checkpoint holds, named as checkpoint.state_spec names them.  The bf16 compute
+        copies are not among them (re-derived on load), nor the gradient (zeroed by the optimiser at every step)."""
+        st = self.store
+        out = {}
+        for prefix, view in (("param", st.f32), ("exp_avg", st.exp_avg), ("exp_avg_sq", st.exp_avg_sq)):
+            out.update({f"{prefix}/{e.name}": view(e.name) for e in self.table})
+        out.update({f"teacher/{e.name}": st.tf32(e.name) for e in self.table if e.teacher})
+        out["center/dino"], out["center/ibot"] = self.center_dino, self.center_ibot
+        out["optimizer/hyper"] = self.hyper[0:3]      # step, 1 - beta1^step, 1 - beta2^step
+        return out
+
+    @torch.no_grad()
+    def save_checkpoint(self, path: str, pipeline=None) -> None:
+        """Write the whole training state at a step boundary into the directory `path` (atomically, see checkpoint.py):
+        fp32 master weights, Adam moments, EMA teacher, DINO / iBOT centres, the optimiser step, this rank's CUDA
+        generator (stochastic-depth subsets) and, given `pipeline` (data.TrainBatchPipeline), its RNG streams.  Every
+        rank calls it.  Settings are not state: learning rate, weight decay, momentum and their schedules come from the
+        code that resumes; the configs are recorded in the manifest only."""
+        import dataclasses
+
+        from . import checkpoint as C
+        torch.cuda.current_stream(self.device).synchronize()
+        C.save(path, self._checkpoint_tensors(), step=self.step_count, cuda_rng=torch.cuda.get_rng_state(self.device),
+               pipeline=None if pipeline is None else pipeline.state_dict(),
+               config={"model": self.cfg.to_dict(), "train": dataclasses.asdict(self.tc)},
+               rank=self.rank, world=self.world, process_group=self.pg)
+
+    @torch.no_grad()
+    def load_checkpoint(self, path: str, rng: bool = True, pipeline=None) -> int:
+        """Restore what save_checkpoint wrote, in place: every buffer is overwritten by copy_, none is rebound, so a
+        step graph captured before the load replays from the restored state.  The whole checkpoint is validated first;
+        a mismatch (another preset, another head_out_dim, ...) raises ValueError and changes nothing.  rng=False skips
+        the per-rank RNG state: the way to resume on another number of GPUs (the rest of the state does not depend on
+        the world size).  Given `pipeline`, its RNG streams are restored too.  Returns the restored step."""
+        from . import checkpoint as C
+        spec = C.state_spec(self.table, self.tc.head_out_dim)
+        ck = C.load(path, spec, rank=self.rank, world=self.world, rng=rng, pipeline=pipeline is not None)
+        if pipeline is not None:
+            pipeline.check_loadable()
+        torch.cuda.current_stream(self.device).synchronize()
+        for name, view in self._checkpoint_tensors().items():
+            view.copy_(ck.tensor(name))
+        st = self.store
+        st.g.zero_()                                      # as at any step boundary
+        lib.cast_f32_to_bf16(st.p, st.pb, st.n)          # the bf16 copies, as the fused optimiser rounds them
+        if st.n_teacher:
+            lib.cast_f32_to_bf16(st.tp, st.tpb, st.n_teacher)
+        self.step_count = ck.step
+        if rng:
+            torch.cuda.set_rng_state(ck.cuda_rng, self.device)
+        if pipeline is not None:
+            pipeline.load_state_dict(ck.pipeline)
+        torch.cuda.current_stream(self.device).synchronize()
+        return ck.step
 
     # -------------------------------------------------------------- pieces shared by the objectives
     def _drop(self, ratio: float):
