@@ -105,10 +105,10 @@ def test_load_into_captured_graph(tmp_path):
     la = [a.train_step(x).cpu().clone() for x in seq]       # the uninterrupted run, from the saved RNG state
     b = _trainer(1)
     b.capture_step(batch, warmup=2)
-    graph, launches = b._graph, b.graph_launches
+    graph, launches = b._graph.graph, b.graph_launches
     b.load_checkpoint(path)
     _assert_same(saved, b)
-    assert b._graph is graph
+    assert b._graph.graph is graph
     lb = [b.replay_step(x).cpu().clone() for x in seq]
     _assert_track(la, lb, a, b)
     assert b.scheduled_values() == a.scheduled_values()

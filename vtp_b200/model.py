@@ -30,6 +30,7 @@ from . import engine as E
 from . import lib
 from . import params as P
 from .config import VTPConfig
+from .graphs import StepGraph
 from .rope import rope_periods
 
 BF = torch.bfloat16
@@ -112,45 +113,36 @@ class VTPModel(VTPPreTrainedModel):
         self.reset_parameters()
         self._packs: Dict[Tuple[str, str], Tuple[int, E.TowerW]] = {}
         self._graphs_on = False          # see enable_cuda_graphs()
-        self._graph_busy = False         # True while a graph is being warmed up / captured (the eager path runs)
         self._graphs: Dict[tuple, tuple] = {}
 
     # ------------------------------------------------------------------ CUDA graphs for the inference entry points
     def enable_cuda_graphs(self, on: bool = True):
         """Replay captured CUDA graphs for get_reconstruction_latents / get_latents_decoded_images /
         get_clip_image_feature / get_clip_text_feature (one graph per input shape, dtype and precision mode; dropped
-        when the parameters change).  Results are identical to the eager launches: the same kernels in the same order."""
+        when the parameters change).  Results are identical to the eager launches: the same kernels in the same order.
+        A call made while the current stream is capturing (an evaluator's whole step) runs its kernels into that capture."""
         self._graphs_on = bool(on)
         if not on:
-            self._graphs = {}
+            self._drop_graphs()
         return self
 
-    def _graphed(self, name: str, fn, x: torch.Tensor, *extra):
-        """Run fn(x) through a captured graph: static input buffer <- x, replay, fresh copy of the static output."""
-        if not x.is_cuda:
-            raise lib.VtpError("VTPModel inputs must live on the CUDA device (no CPU path)")
+    def _drop_graphs(self):
+        for _, graph, _, _ in self._graphs.values():
+            graph.release()
+        self._graphs = {}
+
+    def _graphed(self, name: str, body, x: torch.Tensor, *extra):
+        """body(x), or with graphs on: static input buffer <- x, replay of body's graph, fresh copy of the static output."""
+        if not (self._graphs_on and x.is_cuda) or torch.cuda.is_current_stream_capturing():
+            return body(x)
         key = (name, tuple(x.shape), x.dtype, self._mode(), extra)
         ver = self._version()
         hit = self._graphs.get(key)
         if hit is None or hit[0] != ver:
             static_in = x.detach().clone()
-            cur = torch.cuda.current_stream()
-            side = torch.cuda.Stream()
-            side.wait_stream(cur)
-            self._graph_busy = True
-            try:
-                with torch.cuda.stream(side):    # warm-up: packs the weights, builds RoPE tables, sizes the allocator
-                    for _ in range(2):
-                        fn(static_in)
-                cur.wait_stream(side)
-                torch.cuda.synchronize()
-                graph = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(graph):
-                    static_out = fn(static_in)
-            finally:
-                self._graph_busy = False
-            hit = (ver, graph, static_in, static_out)
-            self._graphs[key] = hit
+            graph = StepGraph(x.device)         # warm-up: packs the weights, builds RoPE tables, sizes the allocator
+            static_out = graph.capture(lambda: body(static_in), warmup=2)
+            hit = self._graphs[key] = (ver, graph, static_in, static_out)
         _, graph, static_in, static_out = hit
         static_in.copy_(x)
         graph.replay()
@@ -350,12 +342,12 @@ class VTPModel(VTPPreTrainedModel):
 
     def invalidate_packed_weights(self):
         self._packs = {}
-        self._graphs = {}
+        self._drop_graphs()
 
     def _apply(self, fn, *args, **kwargs):     # .to() / .cuda() / .half(): packed copies and graphs point at the old storage
         out = super()._apply(fn, *args, **kwargs)
         if hasattr(self, "_packs"):
-            self._packs, self._graphs = {}, {}
+            self.invalidate_packed_weights()
         return out
 
     def _pack(self, tower: str, mode: str) -> E.TowerW:
@@ -427,9 +419,9 @@ class VTPModel(VTPPreTrainedModel):
     def get_clip_image_feature(self, image: torch.Tensor, normalize: bool = True) -> torch.Tensor:
         if self.visual_proj is None:
             raise RuntimeError("CLIP not enabled. Set train_clip=True in config.")
-        if self._graphs_on and image.is_cuda and not self._graph_busy:
-            self._check_image(image)
-            return self._graphed("clip_image", lambda t: self.get_clip_image_feature(t, normalize), image, normalize)
+        return self._graphed("clip_image", lambda t: self._clip_image_feature(t, normalize), image, normalize)
+
+    def _clip_image_feature(self, image: torch.Tensor, normalize: bool) -> torch.Tensor:
         mode = self._mode()
         out, meta, W = self._trunk(image, not self.config.vision_bottleneck_ae_only, mode)
         if self.config.vision_clip_feat == "cls":
@@ -452,8 +444,9 @@ class VTPModel(VTPPreTrainedModel):
             raise RuntimeError("CLIP not enabled. Set train_clip=True in config.")
         if text.dtype != torch.int64 or text.dim() != 2 or text.shape[1] != self.config.text_context_length:
             raise ValueError(f"expected int64 token ids of shape (B, {self.config.text_context_length})")
-        if self._graphs_on and text.is_cuda and not self._graph_busy:
-            return self._graphed("clip_text", lambda t: self.get_clip_text_feature(t, normalize), text, normalize)
+        return self._graphed("clip_text", lambda t: self._clip_text_feature(t, normalize), text, normalize)
+
+    def _clip_text_feature(self, text: torch.Tensor, normalize: bool) -> torch.Tensor:
         mode = self._mode()
         W = self._pack("text", mode)
         f = E.text_forward(W, text, mode)
@@ -485,9 +478,9 @@ class VTPModel(VTPPreTrainedModel):
         return logits, logits.T
 
     def get_reconstruction_latents(self, image: torch.Tensor) -> torch.Tensor:
-        if self._graphs_on and image.is_cuda and not self._graph_busy:
-            self._check_image(image)
-            return self._graphed("latents", self.get_reconstruction_latents, image)
+        return self._graphed("latents", self._reconstruction_latents, image)
+
+    def _reconstruction_latents(self, image: torch.Tensor) -> torch.Tensor:
         out, meta, _ = self._trunk(image, True, self._mode())
         _, _, gh, gw = meta
         pt = out["x_norm_patchtokens"]
@@ -501,8 +494,9 @@ class VTPModel(VTPPreTrainedModel):
             raise RuntimeError("Reconstruction not enabled. Set train_reconstruction=True in config.")
         if not latents.is_cuda:
             raise lib.VtpError("VTPModel inputs must live on the CUDA device (no CPU path)")
-        if self._graphs_on and latents.is_cuda and not self._graph_busy:
-            return self._graphed("decode", self.get_latents_decoded_images, latents)
+        return self._graphed("decode", self._decoded_images, latents)
+
+    def _decoded_images(self, latents: torch.Tensor) -> torch.Tensor:
         mode = self._mode()
         return E.decoder_forward(self._pack("decoder", mode), latents, mode)
 

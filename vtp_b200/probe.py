@@ -29,6 +29,7 @@ import torch
 
 from . import engine as E
 from . import lib
+from .graphs import StepGraph
 
 F32, BF = torch.float32, torch.bfloat16
 
@@ -186,7 +187,7 @@ class LinearProbe:
         self.hyper = torch.zeros(8, dtype=F32, device=dev)      # [0] = optimiser steps taken (vtp_hyper_tick)
         self.loss_acc = torch.zeros(G, dtype=F32, device=dev)
         self.step_count = 0
-        self._graph = None
+        self._graph = StepGraph(dev, enabled=use_graph)
         self._static: Optional[Tuple[torch.Tensor, torch.Tensor]] = None
 
     # ------------------------------------------------------------------ buffers
@@ -283,16 +284,7 @@ class LinearProbe:
             raise ValueError(f"train_step: images {tuple(images.shape)}, earlier steps used {tuple(img.shape)}")
         img.copy_(images, non_blocking=True)
         lab.copy_(labels, non_blocking=True)
-        if self.use_graph and self._graph is None and self.step_count >= 1:
-            torch.cuda.synchronize(self.device)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                self.classifier_step(self.features(img), lab)
-            self._graph = graph
-        if self._graph is not None:
-            self._graph.replay()
-        else:
-            self.classifier_step(self.features(img), lab)
+        self._graph(lambda: self.classifier_step(self.features(img), lab))
         self.step_count += 1
 
     def take_losses(self) -> torch.Tensor:
@@ -334,10 +326,7 @@ class LinearProbe:
 
     def release(self) -> None:
         """Drop the captured step graph (required before torch.distributed.destroy_process_group())."""
-        if self._graph is not None:
-            torch.cuda.synchronize(self.device)
-            self._graph.reset()
-            self._graph = None
+        self._graph.release()
 
 
 # ---------------------------------------------------------------------------------------------------------- CLI

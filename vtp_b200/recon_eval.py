@@ -27,6 +27,7 @@ from typing import Dict, List, Optional
 import torch
 
 from . import lib
+from .graphs import StepGraph
 
 F32 = torch.float32
 IMAGENET_DEFAULT_MEAN = (0.485, 0.456, 0.406)
@@ -71,7 +72,7 @@ def rank_mean(values_mean: Optional[float], world: int, device) -> Optional[floa
 class _Step:
     """Device buffers of one batch shape (the graph's static inputs and outputs)."""
 
-    def __init__(self, B: int, H: int, W: int, dev, lpips: bool, save: bool, fid: bool = False):
+    def __init__(self, B: int, H: int, W: int, dev, lpips: bool, save: bool, fid: bool, use_graph: bool):
         self.x = torch.empty((B, 3, H, W), dtype=F32, device=dev)
         self.nbands = min(H, 16)
         self.sse = torch.empty((B, self.nbands), dtype=torch.float64, device=dev)
@@ -82,8 +83,7 @@ class _Step:
         self.lp = torch.empty((B, 2, 3, H, W), dtype=F32, device=dev) if lpips else None
         self.u8 = torch.empty((2, B, H, W, 3), dtype=torch.uint8, device=dev) if save else None
         self.fid_rows = torch.zeros(1, dtype=torch.int32, device=dev) if fid else None  # images of the batch with a PNG
-        self.graph = None
-        self.seen = 0
+        self.graph = StepGraph(dev, enabled=use_graph)
         self.copied = None   # event: the last PNG copy out of u8 has finished
 
 
@@ -181,24 +181,14 @@ class ReconstructionEvaluator:
         st = self._steps.get(key)
         if st is None:
             st = self._steps[key] = _Step(B, H, W, self.device, self.lpips is not None, self.save_dir is not None,
-                                          self.fid is not None)
+                                          self.fid is not None, self.use_graph)
         if st.copied is not None:
             torch.cuda.current_stream(self.device).wait_event(st.copied)  # the last batch's PNG copy has left st.u8
         st.x.copy_(images, non_blocking=True)
         idx = png_indices(self.batches, self.batch_size, self.world, self.rank, B, self.total) if self.save_dir else []
         if st.fid_rows is not None:
             st.fid_rows.fill_(len(idx))
-        if self.use_graph and st.graph is None and st.seen >= 1:
-            torch.cuda.synchronize(self.device)
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self._run(st)
-            st.graph = g
-        if st.graph is not None:
-            st.graph.replay()
-        else:
-            self._run(st)
-        st.seen += 1
+        st.graph(lambda: self._run(st))
         self._psnr.append(st.psnr.clone())
         self._ssim.append(st.ssim.clone())
         if st.lpips is not None:
@@ -266,10 +256,7 @@ class ReconstructionEvaluator:
             self._pool.shutdown(wait=True)
             self._pool = None
         for st in self._steps.values():
-            if st.graph is not None:
-                torch.cuda.synchronize(self.device)
-                st.graph.reset()
-                st.graph = None
+            st.graph.release()
 
 
 def _write_pngs(done, host, idx, ref_dir, rec_dir) -> None:

@@ -26,6 +26,7 @@ from . import lib
 from . import params as P
 from .config import VTPConfig
 from .engine import BF, F32, BlockW, Lin, TowerW, _e
+from .graphs import StepGraph
 from .rope import rope_periods
 
 _ALIGN = 64  # elements; keeps every tensor 128B-aligned in the bf16 copy (TMA needs 16B)
@@ -960,20 +961,10 @@ class VTPTrainer:
             ps = self.cfg.vision_patch_size
             HW = (batch["global_crops"].shape[-2] // ps) * (batch["global_crops"].shape[-1] // ps)
             self._static.update(self.split_masks(self._static["mask_indices"], self._static["masks_weight"], B, HW))
-        cur = torch.cuda.current_stream(self.device)
-        side = torch.cuda.Stream(self.device)
-        side.wait_stream(cur)
-        with torch.cuda.stream(side):
-            for _ in range(warmup):
-                self.train_step(self._static)
-        cur.wait_stream(side)
-        torch.cuda.synchronize(self.device)
-        l0 = lib.LAUNCHES
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            self.train_step(self._static)
+        graph = StepGraph(self.device)
+        graph.capture(lambda: self.train_step(self._static), warmup)
         self.step_count -= 1                      # the capture did not execute
-        self.graph_launches = lib.LAUNCHES - l0   # kernels of ours inside one replay
+        self.graph_launches = graph.launches      # kernels of ours inside one replay
         self._graph = graph
         return self
 
@@ -994,7 +985,6 @@ class VTPTrainer:
                 v.copy_(batch[k], non_blocking=True)
         self._graph.replay()
         self.step_count += 1
-        lib.LAUNCHES += self.graph_launches
         return self.loss_acc
 
     def release_graph(self):
@@ -1002,8 +992,7 @@ class VTPTrainer:
         multi-rank job: NCCL does not tear a communicator down while a CUDA graph that captured its collectives is alive
         (the 2-GPU run of round 2 hung in destroy_process_group until the graph was released first)."""
         if self._graph is not None:
-            torch.cuda.synchronize(self.device)
-            self._graph.reset()
+            self._graph.release()
             self._graph = None
             self._static = None
             import gc

@@ -29,6 +29,7 @@ import torch
 
 from . import engine as E
 from . import lib
+from .graphs import StepGraph
 
 F32, BF = torch.float32, torch.bfloat16
 IMAGENET_DEFAULT_MEAN = (0.485, 0.456, 0.406)
@@ -242,7 +243,7 @@ def accuracy_from_ranks(ranks: np.ndarray, topk: Sequence[int] = (1, 5)) -> List
 class _Step:
     """Device buffers of one batch shape (the graph's static inputs and outputs)."""
 
-    def __init__(self, B: int, H: int, W: int, E: int, Cp: int, mode: str, dev):
+    def __init__(self, B: int, H: int, W: int, E: int, Cp: int, mode: str, dev, use_graph: bool):
         act = BF if mode == "bf16" else F32
         self.x = torch.empty((B, 3, H, W), dtype=act, device=dev)
         self.t = torch.empty(B, dtype=torch.int64, device=dev)
@@ -250,8 +251,7 @@ class _Step:
         self.a3 = torch.empty((B, 3 * E), dtype=BF, device=dev) if mode == "fp32" else None
         self.logits = torch.empty((B, Cp), dtype=act, device=dev)
         self.ranks = torch.empty(B, dtype=torch.int32, device=dev)
-        self.graph = None
-        self.seen = 0
+        self.graph = StepGraph(dev, enabled=use_graph)
 
 
 class ZeroShotEvaluator:
@@ -294,12 +294,12 @@ class ZeroShotEvaluator:
     # ------------------------------------------------------------------ the device step
     def _run(self, st: _Step) -> None:
         m = self.model
-        saved = m.compute_mode, m._graphs_on
+        saved = m.compute_mode
         try:
-            m.compute_mode, m._graphs_on = self.mode, False   # this step is captured whole: no nested per-call graphs
+            m.compute_mode = self.mode
             f = m.get_clip_image_feature(st.x, normalize=False)
         finally:
-            m.compute_mode, m._graphs_on = saved
+            m.compute_mode = saved
         if f.shape[1] != self.E:
             raise ValueError(f"image features have width {f.shape[1]}, the classifier {self.E}")
         self.head(st, f.contiguous())
@@ -327,19 +327,10 @@ class ZeroShotEvaluator:
         key = (B, H, W)
         st = self._steps.get(key)
         if st is None:
-            st = self._steps[key] = _Step(B, H, W, self.E, self.Cp, self.mode, self.device)
+            st = self._steps[key] = _Step(B, H, W, self.E, self.Cp, self.mode, self.device, self.use_graph)
         st.x.copy_(images, non_blocking=True)
         st.t.copy_(targets, non_blocking=True)
-        if self.use_graph and st.graph is None and st.seen >= 1:
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self._run(st)
-            st.graph = g
-        if st.graph is not None:
-            st.graph.replay()
-        else:
-            self._run(st)
-        st.seen += 1
+        st.graph(lambda: self._run(st))
         self.n += B
         self._ranks.append(st.ranks.clone())
 
@@ -359,10 +350,7 @@ class ZeroShotEvaluator:
 
     def close(self) -> None:
         for st in self._steps.values():
-            if st.graph is not None:
-                torch.cuda.synchronize(self.device)
-                st.graph.reset()
-                st.graph = None
+            st.graph.release()
 
 
 def evaluate(model, classifier: torch.Tensor, dataloader, device, precision: str = "fp32") -> Tuple[float, float]:
